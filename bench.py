@@ -1,16 +1,18 @@
 #!/usr/bin/env python
 """bench.py — headline benchmark of the hot path (contract: see DESIGN.md §Measurement).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 metric  : SE3 Exp+Log Mops/s (1 op = one se3->SE3 Exp plus one SE3->se3 Log on one element)
 workload: BASELINE.json configs[1] — batch 10^6, fp32, per GPU (weak scaling, no data-path collective)
 step    : one Exp launch + one Log launch over one resident batch; batches rotate through a ring whose
-          footprint exceeds the 126 MB L2 (Log reads the SE3 batch Exp just wrote, possibly still in L2; nothing else is).
+          footprint exceeds the 50 MB L2 of the H100 (Log reads the SE3 batch Exp just wrote, possibly still in L2; nothing else is).
 value   : device-timed (CUDA events, max over ranks), inputs resident in HBM; W warm-up steps, then exactly K steps between
           barrier + synchronize pairs, repeated REGIONS times, median region reported.
 legs    : LM step/s (PoseInv, reprojection at 1e6 / 1e7 / 2e8 residual rows, pose graph, bundle adjustment) and IMU
           Msamples/s through the public API, each with its own roofline object (bench_legs.py).
+outputs : --dump-outputs DIR writes what the last timed step computed (rank 0), float32: DIR/SE3_exp.npy (n, 7) and
+          DIR/se3_log.npy (n, 6).  The inputs are seeded, so two builds run with the same arguments compare output for output.
 e2e     : same metric through the public API (pp.se3(...).Exp().Log()) with pinned HOST buffers,
           H2D and D2H copies inside the timed region.
 The reference arm (--impl reference) times the torch-CPU port of the reference's Exp/Log op
@@ -39,7 +41,7 @@ sys.path.insert(0, ROOT)
 BATCH = 1_000_000
 BYTES_EXP = 4 * (6 + 7)      # algorithmic bytes / element (SURVEY.md §8d): read se3 (24) + write SE3 (28)
 BYTES_LOG = 4 * (7 + 6)
-L2_BYTES = 126 * 2 ** 20
+L2_BYTES = 50 * 2 ** 20      # H100 SXM
 METRIC = "SE3 Exp+Log throughput (batch 1e6, fp32)"
 UNIT = "Mops/s"
 
@@ -49,7 +51,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -155,7 +157,7 @@ def run_ours(args):
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
     n = BATCH
-    ring = 8                                  # 8 x 76 MB = 608 MB of distinct buffers, > 4 x L2
+    ring = 8                                  # 8 x 76 MB = 608 MB of distinct buffers, > 12 x L2
     xs = [se3_batch(n, 1234 + 100 * rank + j, dev) for j in range(ring)]
     Xs = [torch.empty(n, 7, device=dev) for _ in range(ring)]
     ys = [torch.empty(n, 6, device=dev) for _ in range(ring)]
@@ -215,6 +217,8 @@ def run_ours(args):
         ms = timed_region(graphs, K)
         barrier(world)
         regions.append(max_over_ranks(ms, world, dev))
+    if args.dump_outputs and rank == 0:      # the last timed step ran on ring slot (K - 1) % ring (see timed_region)
+        dump_outputs(args.dump_outputs, {"SE3_exp": Xs[(K - 1) % ring], "se3_log": ys[(K - 1) % ring]})
     # keep the GPU busy long enough for nvidia-smi to see clocks under load (a 0.4 ms region is shorter than one sample)
     t_end = time.perf_counter() + 0.35
     while time.perf_counter() < t_end:
@@ -236,7 +240,7 @@ def run_ours(args):
     ach = n * b_dom / (t_dom * 1e-3) / 1e9
     step_gbs = n * (BYTES_EXP + BYTES_LOG) / (ms_per_step * 1e-3) / 1e9
     roofline = {"bound": "hbm", "kernel": f"stream_kernel_tma<{dom}>", "achieved": round(ach, 1), "peak": peak,
-                "unit": "GB/s", "frac": round(ach / peak, 4), "traffic": TRAFFIC.get(dom), "peak_source": peak_src,
+                "unit": "GB/s", "frac": round(ach / peak, 4), "peak_source": peak_src,
                 "bytes_per_launch": n * b_dom, "us_per_launch": round(t_dom * 1e3, 2), "exp_us": round(t_exp * 1e3, 2),
                 "log_us": round(t_log * 1e3, 2), "step_gbs": round(step_gbs, 1), "step_frac": round(step_gbs / peak, 4)}
 
@@ -294,7 +298,8 @@ def run_ours(args):
     if rank == 0:
         cfg = base_config(world)
         cfg.update({"launch": "CUDA graphs: K // 8 trips of an 8-step graph + K % 8 single-step graphs", "timed_regions": REGIONS,
-                    "l2": f"inputs larger than L2: ring of {ring} batches, footprint {footprint >> 20} MiB > 126 MiB L2"})
+                    "l2": f"inputs larger than L2: ring of {ring} batches, footprint {footprint >> 20} MiB > "
+                          f"{L2_BYTES >> 20} MiB L2"})
         line = {"metric": METRIC, "value": round(value, 1), "unit": UNIT, "n_gpus": world, "steps": K, "warmup": W,
                 "ms_per_step": round(ms_per_step, 6), "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "f32", "data": "synthetic", "gpu_launches": 2 * K}
@@ -308,13 +313,14 @@ def run_ours(args):
 
 REGIONS = 5
 
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full capture
-# (profiles/); None until measured.
-TRAFFIC = {}
-try:
-    TRAFFIC = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-except (OSError, ValueError):
-    pass
+
+def dump_outputs(out_dir, arrays):
+    """arrays: name -> tensor; each written as out_dir/<name>.npy (float32 stays float32, everything else float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), a if a.dtype == np.float32 else a.astype(np.float64))
 
 
 def usable_cores():
@@ -405,6 +411,7 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-large", dest="no_large", action="store_true", help="skip the 2e8-residual LM leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

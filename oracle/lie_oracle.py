@@ -9,8 +9,8 @@ Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may import 
 The shipped package (pypose_b200/) never does: it has no CPU path at all.
 
 Parity of this oracle is pinned by tests/test_oracle_golden.py against tests/golden/*.npz, which
-were produced by importing the reference itself (oracle/make_golden.py, run in the build
-container where /root/reference exists).
+were produced by importing the reference itself (oracle/make_golden.py, run against the
+reference checkout named by PYPOSE_REFERENCE).
 
 Entry point: run(symbol, *arrays) with the same names / argument order as the C-ABI
 (include/b200pose.h) minus the `b200_` prefix and dtype suffix, e.g. run("SE3_log_bwd", x, g).

@@ -1,9 +1,9 @@
 """Generate golden vectors by running the REFERENCE itself (pypose v0.9.5 imported from
-/root/reference) in fp64 on CPU.  Run in the build container only:
+the checkout named by PYPOSE_REFERENCE) in fp64 on CPU:
 
     python oracle/make_golden.py            # writes tests/golden/lie_ops.npz
 
-The GPU box has no /root/reference; the committed .npz travels instead.  Inputs are seeded; every
+The tests read only the committed .npz, never the reference.  Inputs are seeded; every
 (group, op) gets N_RANDOM random rows plus hand-placed edge rows (identity, tiny / near-pi angles,
 negative-w quaternions).  Backward goldens come from the reference's own autograd.
 """
@@ -13,7 +13,7 @@ import sys
 import numpy as np
 import torch
 
-REF = os.environ.get("PYPOSE_REFERENCE", "/root/reference")
+REF = os.environ["PYPOSE_REFERENCE"]
 sys.path.insert(0, REF)
 sys.dont_write_bytecode = True
 import pypose as ref  # noqa: E402

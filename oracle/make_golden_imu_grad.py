@@ -10,7 +10,7 @@ import sys
 import numpy as np
 import torch
 
-sys.path.insert(0, os.environ.get("PYPOSE_REFERENCE", "/root/reference"))
+sys.path.insert(0, os.environ["PYPOSE_REFERENCE"])
 sys.dont_write_bytecode = True
 import pypose as ref  # noqa: E402
 

@@ -12,7 +12,7 @@ import numpy as np
 import torch
 from torch import nn
 
-sys.path.insert(0, os.environ.get("PYPOSE_REFERENCE", "/root/reference"))
+sys.path.insert(0, os.environ["PYPOSE_REFERENCE"])
 sys.dont_write_bytecode = True
 import pypose as ref  # noqa: E402
 

@@ -1,8 +1,8 @@
-"""pypose_b200 — a B200-native implementation of PyPose's data-parallel core.
+"""pypose_b200 — an H100-native implementation of PyPose's data-parallel core.
 
 `import pypose_b200 as pp` exposes the hot-path surface of pypose v0.9.5 (LieTensor op family,
 pp.optim LM/GN inner loop, IMU preintegration scan) with every numeric operator implemented as a
-hand-written sm_100a CUDA kernel behind a C-ABI library (include/b200pose.h).  There is no CPU
+hand-written sm_90a CUDA kernel behind a C-ABI library (include/b200pose.h).  There is no CPU
 fallback: operators on CPU tensors raise.
 """
 import torch

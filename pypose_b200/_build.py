@@ -1,8 +1,8 @@
-"""In-tree build of libb200pose.so (sm_100a only).
+"""In-tree build of libb200pose.so (sm_90a, H100, only).
 
 `python -m pypose_b200._build` or `__graft_entry__.build()`.  nvcc cross-compiles without a GPU.
-Objects are cached under pypose_b200/csrc/build/ keyed on source mtimes; the shared library is
-written to pypose_b200/lib/ so that it travels with the repo snapshot to the GPU box.
+Objects are cached under pypose_b200/csrc/build/ keyed on source mtimes and the compile flags; the shared
+library is written to pypose_b200/lib/, where pypose_b200._C loads it from the source tree.
 """
 import os
 import subprocess
@@ -15,10 +15,8 @@ OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(HERE, "lib", "libb200pose.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-    "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",
-]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
 def _sources():
@@ -54,18 +52,25 @@ def _compile(src, hm, verbose):
 def build(verbose=False, force=False):
     os.makedirs(OBJ, exist_ok=True)
     os.makedirs(os.path.dirname(LIB), exist_ok=True)
-    hm = float("inf") if force else _headers_mtime()
+    stamp = os.path.join(OBJ, "flags.txt")
+    key = " ".join([NVCC] + FLAGS)
+    if not force and (not os.path.exists(stamp) or open(stamp).read() != key):
+        force = True                       # objects built with other flags (another architecture) are not reused
     if force:
         for f in os.listdir(OBJ):
             os.remove(os.path.join(OBJ, f))
-        hm = _headers_mtime()
+        if os.path.exists(LIB):
+            os.remove(LIB)
+        with open(stamp, "w") as f:
+            f.write(key)
+    hm = _headers_mtime()
     srcs = _sources()
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         res = list(ex.map(lambda s: _compile(s, hm, verbose), srcs))
     objs = [o for o, _ in res]
     changed = any(c for _, c in res)
     if changed or not os.path.exists(LIB) or os.path.getmtime(LIB) < max(os.path.getmtime(o) for o in objs):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ARCH
         if verbose:
             print(" ".join(cmd), flush=True)
         r = subprocess.run(cmd, capture_output=True, text=True)

@@ -1,9 +1,8 @@
 // ba.cu — bundle adjustment without atomics: bit-reproducible block sums (C-ABI: include/b200pose.h, section LM).
 //
-// Round-1 finding (VERDICT r1, GPUTEST_r01 smoke): the camera-side sums of the BA route were scatter-added with
-// warp-aggregated atomics, so Hcc / gc / the Schur diagonal / every W v product depended on the order in which warps
-// reached the atomic unit.  On an ill-conditioned fp32 system that noise seeded a chaotic CG (30 different outcomes in
-// 30 runs of the same seeded problem, profiles/r2a_spread.log).  Here every sum has ONE writer and a fixed order:
+// Scatter-added with warp-aggregated atomics, the camera-side sums of the BA route (Hcc / gc / the Schur diagonal / every
+// W v product) depend on the order in which warps reach the atomic unit.  On an ill-conditioned fp32 system that noise
+// seeds a chaotic CG (different outcomes from run to run of the same seeded problem).  Here every sum has ONE writer and a fixed order:
 //
 //  * observations are grouped by camera once (optim/structured.py BAProblem), cseg[c] .. cseg[c+1] are camera c's rows;
 //  * a work item is (camera c, sub-range s of S): TPI threads (one warp, or one 128-thread CTA) stride over the item's

@@ -111,7 +111,7 @@ __global__ void __launch_bounds__(kThreads) stream_kernel(StreamParams<typename 
 // shared-memory ring signalled by mbarriers, bulk stores back (cp.async.bulk.global.shared).
 // One elected thread issues all copies, so the other threads spend their issue slots on math only
 // and loads for tile i+S overlap the math of tile i *inside* a CTA (v1 relies on other CTAs for that,
-// which fails when a single wave of CTAs runs in lock-step: ncu profiles/r1a).
+// which fails when a single wave of CTAs runs in lock-step).
 // Requirements: all base pointers 16 B aligned and every tile a multiple of 4 elements (the launcher
 // guarantees both; the <= 3 element remainder and unaligned tensors go through the v1 kernel).
 // ----------------------------------------------------------------------------

@@ -68,7 +68,7 @@ LM_HD void m_sincos(double x, double& s, double& c) {
 
 // Reciprocal and reciprocal square root.  fp32 on the device: one MUFU approximation + one Newton step
 // (~1 ulp, 3-4 instructions, no branches) instead of the IEEE division / sqrt sequences whose
-// denormal fix-up paths cost ~10 extra instructions and a divergent branch each (ncu profiles/r1a).
+// denormal fix-up paths cost ~10 extra instructions and a divergent branch each.
 // x = 0 yields inf/NaN exactly like 1/x would; callers select those lanes away.
 LM_HD float m_rcp(float x) {
 #if defined(__CUDA_ARCH__)

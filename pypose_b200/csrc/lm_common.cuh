@@ -51,8 +51,7 @@ __device__ __forceinline__ bool reduce_sums(double (&v)[NS], double* ws) {
     __threadfence();
     // Fixed-order fold by the whole CTA: thread-strided partial sums with the loads of kFold CTAs' partials issued before
     // the first add, then the shuffle tree and a fixed-order sum of the warp results.  (The one-warp, one-load-at-a-time loop
-    // this replaces walked grid/32 dependent L2 round trips; measured r2h -> r2j the change is worth ~1 us per launch at
-    // 625-1184 CTAs — the kernels that end with this reduction are bound elsewhere.)
+    // this replaces walked grid/32 dependent L2 round trips.)
     constexpr int kFold = 4;
     double t[NS];
 #pragma unroll

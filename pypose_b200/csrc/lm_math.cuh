@@ -404,55 +404,14 @@ template <typename T> LM_HD void sym3_unpack(const T* a, T (&A)[3][3]) {
 
 
 
-// ---------------------------------------------------------------- J^T J accumulator (Blackwell packed fp32)
-// Acc6<T>: the running 6x6 system of a thread.  For float the 21 + 6 accumulators are updated with `fma.rn.f32x2`
-// (SASS FFMA2, two fp32 FMAs per issue slot): the upper triangle is held as the pairs (a, b), (a, b+1) that start at even
-// b, the three odd diagonal entries stay scalar -> 12 FFMA2 + 3 FFMA per Jacobian row instead of 27 FFMA.  Round-1 ncu
-// (profiles/r1h_lm_large_ncu_full_summary.csv) had the accumulate kernel issue-bound on exactly those FMAs, with zero
-// FFMA2 in its SASS.  Same products, same summation order per accumulator => bit-identical to sys6_add_row.
+// ---------------------------------------------------------------- J^T J accumulator
+// Acc6<T>: the running 6x6 system of a thread (21 + 6 scalar FMAs per Jacobian row; sm_90 has no packed fp32 FMA).
 template <typename T> struct Acc6 {
   Sys6<T> s;
   LM_HD void zero() { sys6_zero(s); }
   LM_HD void add_row(const T (&j)[6], T r) { sys6_add_row(s, j, r); }
   LM_HD Sys6<T> finish() const { return s; }
 };
-#if defined(__CUDA_ARCH__) && __CUDA_ARCH__ >= 1000
-template <> struct Acc6<float> {
-  float2 p0[3], p1[2], p2[2], p3[1], p4[1], g[3];
-  float s1, s3, s5;
-  __device__ __forceinline__ void zero() {
-    const float2 z = make_float2(0.f, 0.f);
-    p0[0] = p0[1] = p0[2] = p1[0] = p1[1] = p2[0] = p2[1] = p3[0] = p4[0] = g[0] = g[1] = g[2] = z;
-    s1 = s3 = s5 = 0.f;
-  }
-  __device__ __forceinline__ void add_row(const float (&j)[6], float r) {
-    const float2 q0 = make_float2(j[0], j[1]), q1 = make_float2(j[2], j[3]), q2 = make_float2(j[4], j[5]);
-    const float2 a0 = make_float2(j[0], j[0]), a1 = make_float2(j[1], j[1]), a2 = make_float2(j[2], j[2]);
-    const float2 a3 = make_float2(j[3], j[3]), a4 = make_float2(j[4], j[4]), rr = make_float2(r, r);
-    p0[0] = __ffma2_rn(a0, q0, p0[0]); p0[1] = __ffma2_rn(a0, q1, p0[1]); p0[2] = __ffma2_rn(a0, q2, p0[2]);
-    s1 = fmaf(j[1], j[1], s1);
-    p1[0] = __ffma2_rn(a1, q1, p1[0]); p1[1] = __ffma2_rn(a1, q2, p1[1]);
-    p2[0] = __ffma2_rn(a2, q1, p2[0]); p2[1] = __ffma2_rn(a2, q2, p2[1]);
-    s3 = fmaf(j[3], j[3], s3);
-    p3[0] = __ffma2_rn(a3, q2, p3[0]);
-    p4[0] = __ffma2_rn(a4, q2, p4[0]);
-    s5 = fmaf(j[5], j[5], s5);
-    g[0] = __ffma2_rn(rr, q0, g[0]); g[1] = __ffma2_rn(rr, q1, g[1]); g[2] = __ffma2_rn(rr, q2, g[2]);
-  }
-  __device__ __forceinline__ Sys6<float> finish() const {
-    Sys6<float> s;
-    sys6_zero(s);
-    s.A[0][0] = p0[0].x; s.A[0][1] = p0[0].y; s.A[0][2] = p0[1].x; s.A[0][3] = p0[1].y; s.A[0][4] = p0[2].x; s.A[0][5] = p0[2].y;
-    s.A[1][1] = s1; s.A[1][2] = p1[0].x; s.A[1][3] = p1[0].y; s.A[1][4] = p1[1].x; s.A[1][5] = p1[1].y;
-    s.A[2][2] = p2[0].x; s.A[2][3] = p2[0].y; s.A[2][4] = p2[1].x; s.A[2][5] = p2[1].y;
-    s.A[3][3] = s3; s.A[3][4] = p3[0].x; s.A[3][5] = p3[0].y;
-    s.A[4][4] = p4[0].x; s.A[4][5] = p4[0].y;
-    s.A[5][5] = s5;
-    s.g[0] = g[0].x; s.g[1] = g[0].y; s.g[2] = g[1].x; s.g[3] = g[1].y; s.g[4] = g[2].x; s.g[5] = g[2].y;
-    return s;
-  }
-};
-#endif
 
 // ---------------------------------------------------------------- two-pose reprojection (lm.cu lm_reproj2_*)
 // r = proj(T_b^-1 T_a p) - z with proj(y) = (fx y.x/y.z + sk y.y/y.z + cx, fy y.y/y.z + cy); see lm.cu for the citations

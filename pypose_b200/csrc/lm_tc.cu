@@ -1,11 +1,11 @@
 // lm_tc.cu — tensor-core variant of the per-camera J^T J accumulation, kept as the EVIDENCE run that BASELINE.json's
 // north_star asks for ("tensor cores used only where J^T J over a dense residual block is genuinely a large contraction —
-// each choice evidenced by ncu counters ... tensor-pipe % for the J^T J path").  It is NOT on the production path: the
-// measured comparison (profiles/r2*_tc_*.csv, DESIGN.md §3.3) decides, and the scalar kernel wins.
+// each choice evidenced ... tensor-pipe % for the J^T J path").  It is NOT on the production path: the scalar kernel
+// is (DESIGN.md §3.3).
 //
 // Contraction: per camera c with m observations, V = [J | r] is (2m x 7); H = J^T J, g = J^T r and the loss r^T r are the
 // 7x7 Gram matrix V^T V.  K = 2m can be thousands, but M = N = 7: the smallest warp-level tile of the tensor pipe is
-// m16n8k8 (TF32), i.e. at most 7*7 / (16*8) = 38 % of every MMA is useful, and tcgen05's minimum M of 64/128 would waste
+// m16n8k8 (TF32), i.e. at most 7*7 / (16*8) = 38 % of every MMA is useful, and wgmma's minimum M of 64 would waste
 // > 90 % (different cameras have different J, so a block-diagonal batch cannot share one MMA).
 //
 // Layout: one CTA (4 warps) per camera; each lane builds the two rows of its observation in registers, the warp stages

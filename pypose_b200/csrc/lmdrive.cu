@@ -1,9 +1,9 @@
 // lmdrive.cu — native driver of one LM trial for the block-sparse pose families (C-ABI: b200_lm_pgo2_step).
 //
-// Round 2 measured the pose-graph step at ~1.1 ms for ~0.5 ms of kernels: ~15 Python-level launches of 6-8 us each around
-// a PCG loop whose kernels take 5-15 us, plus two blocking reads.  The reference's counterpart is Python too
+// Driven from Python, the pose-graph step spends about as long in ~15 Python-level launches around the PCG loop, plus two
+// blocking reads, as in its kernels.  The reference's counterpart is Python too
 // (optimizer.py:629-680 + the external bae PCG), but here the per-trial sequence is fixed, so it is enqueued from C++ by
-// calling the library's own entry points back to back (~2 us per launch), and the two things the host must learn — "has
+// calling the library's own entry points back to back, and the two things the host must learn — "has
 // the CG finished?" and "was the trial accepted?" — arrive through mapped pinned memory that small kernels publish into.
 #include <string.h>
 #include "lm_common.cuh"

@@ -25,7 +25,7 @@ constexpr int kMaxLmDevices = 64;
 constexpr int kAccRows = 4;          // rows per lane in flight in the register-fed accumulation loops
 
 // The deciding thread also publishes the state in mapped pinned host memory (zero-copy): the host spins on the sequence
-// number instead of paying an asynchronous copy plus a stream synchronisation (~10 us per trial, measured).
+// number instead of paying an asynchronous copy plus a stream synchronisation per trial.
 struct HostOut { double* ptr; double seq; };
 __device__ __forceinline__ void publish_state(const double* st, const HostOut& h) {
   if (!h.ptr) return;
@@ -84,7 +84,7 @@ __global__ void __launch_bounds__(kLmThreads) reproj_trial_kernel(const T* __res
         loss += rho;
       };
       // kAccRows rows per lane in flight: at 96-110 registers only 16-20 warps are resident, so the bytes in flight have
-      // to come from the unroll (2 rows: 26 KB per SM, 0.35 of the HBM peak at 1e7 rows; r2h)
+      // to come from the unroll
       int k = b + sub;
       for (; k + (kAccRows - 1) * LPC < e; k += kAccRows * LPC) {
         T v[kAccRows][5];
@@ -185,7 +185,7 @@ __global__ void __launch_bounds__(kLmThreads) reproj_trial_kernel(const T* __res
 // The same trial with the rows STAGED through shared memory by 1-D TMA bulk copies (tma.cuh): one warp per camera, a ring
 // of kStages tiles of kStageRows rows per warp, each tile one `cp.async.bulk` of the points and one of the pixels signalled
 // by an mbarrier.  The register-fed kernel above keeps (rows in flight per lane) x (resident warps) bytes in flight, and its
-// ~96 registers cap the warps: measured 0.61 of the HBM peak at 2e8 rows.  Here the bytes in flight are the ring
+// ~96 registers cap the warps.  Here the bytes in flight are the ring
 // (kStages x 2.5 KB per warp, ~200 KB per SM), independent of the register count, and the lanes only read shared memory
 // (row stride 3 words / 2 words: conflict-free).  Both passes — accumulate, then the trial loss with the solved pose — are
 // ONE stream of 2 x tiles through the ring, so the first tiles of the second pass are already in flight while the warp
@@ -434,9 +434,8 @@ constexpr int CH_PART = 0, CH_TRIAL = 1, CH_LOSS = 2, CH_POSEINV = 3;
 struct PeerRegions { long long part, pt; };     // byte offsets inside the payload: partial blocks, trial poses
 
 // Exchange slots are padded to whole 16-byte vectors: 28 numbers per (source rank, camera) partial block (21 + 6 + pad),
-// 8 per trial pose.  Every remote store is a 16-byte store and a thread fences ONCE, after its last store (r2l: the first
-// version stored 27 scalars per camera from one lane and issued a system-scope fence per camera — the 2-GPU step took 2.4x
-// the 1-GPU step at 1e6 rows).
+// 8 per trial pose.  Every remote store is a 16-byte store and a thread fences ONCE, after its last store (27 scalar
+// stores per camera from one lane with a system-scope fence per camera made the 2-GPU step slower than the 1-GPU step).
 constexpr int kPartSlot = 28, kPoseSlot = 8;
 
 // K1p: LPC lanes per camera over the local rows (same loop as reproj_trial_kernel), blocks staged in shared memory, then the
@@ -557,8 +556,7 @@ __global__ void __launch_bounds__(kLmThreads) reproj_accum_push_kernel(const T* 
 // Gather form, K2g: every rank holds every rank's partial blocks, adds them in rank order per camera (bit-identical on all
 // ranks), solves, retracts, keeps the block for retries and the trial pose locally, and goes straight on to the trial loss
 // of its local rows — ONE exchange fewer than the owner form (no trial poses travel), at world x the partial-block traffic:
-// chosen when world * ncam blocks are a few MB (r2m: 1e4 cameras / 1e6 rows on 2 GPUs took 98 us per step in the owner form
-// against 54 us on one GPU; three flag waits were most of it).  Predicted reduction / failed pivots are counted by the
+// chosen when world * ncam blocks are a few MB (at 1e4 cameras the owner form's three flag waits dominate the step).  Predicted reduction / failed pivots are counted by the
 // camera's owner only, so that the sums over ranks are the totals.
 template <typename T, int LPC>
 __global__ void __launch_bounds__(kLmThreads) reproj_gather_trial_kernel(

@@ -39,7 +39,7 @@ __device__ __forceinline__ void cg_after_update(double* cg, double rr, double it
 
 // (n, 6) vectors are read and written as three 8-byte (float) / 16-byte (double) pairs: a node's six values start at a
 // multiple of 24 / 48 bytes, so the arrays only have to be 8- / 16-byte aligned (checked at the entry points).  Scalar
-// accesses cost one LSU wavefront per touched line and instruction — 36 per warp and vector instead of 18 (r2j: the PCG
+// accesses cost one LSU wavefront per touched line and instruction — 36 per warp and vector instead of 18 (the PCG
 // kernels are LSU-bound, not DRAM-bound).
 template <typename T> struct Pair6;
 template <> struct Pair6<float> { using type = float2; };
@@ -483,8 +483,8 @@ using namespace b200pose;
 // ---- optional CUDA-graph replay of a chunk of iterations (B200POSE_CG_GRAPH=1; off by default) -----------------------
 // A chunk is 45-90 kernels of 4-20 us each with ~4 us between dependent kernels.  Capturing the chunk once per distinct
 // argument tuple (on a private stream: the caller's stream may be the legacy default stream, which cannot be captured)
-// and replaying it with cudaGraphLaunch was measured on B200 and does NOT help: bundle adjustment 1.63 ms/step with the
-// graph vs 1.58 ms without — the gaps are dependency (drain + launch) latency on the device, not host enqueue cost.
+// and replaying it with cudaGraphLaunch is not expected to help: the gaps are dependency (drain + launch) latency on the
+// device, not host enqueue cost.
 // Kept as an opt-in because it costs nothing when off.  Any failure of the capture API disables it for the process.
 struct GraphCache {
   std::unordered_map<std::string, cudaGraphExec_t> map;

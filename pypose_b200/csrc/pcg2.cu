@@ -1,8 +1,7 @@
 // pcg2.cu — pose-graph / pose-pair PCG without atomics, two kernels per iteration (C-ABI: include/b200pose.h, section LM).
 //
-// Round-1 profile (profiles/r1l_pcg_ncu_full_summary.csv): `lm_pgo_scatter` 7.7 % and `pcg_pgo_spmv` 17 % of HBM peak, both
-// throttled by global fp32 atomics (lg_throttle 287 / 58 stalls per issue), and four kernels per CG iteration with ~4 us
-// between dependent launches.  This file replaces that route on one GPU:
+// The per-edge scatter route (`lm_pgo_scatter`, `pcg_pgo_spmv`) is throttled by global fp32 atomics and needs four kernels
+// per CG iteration.  This file replaces that route on one GPU:
 //
 //  * the per-edge blocks are produced directly in NODE order by the linearisation kernels: every edge (i, j) owns one slot
 //    in i's list and one in j's (epos_i / epos_j), each slot holds the 21 numbers of M_e padded to 24 (96 B, 16-byte

@@ -73,8 +73,7 @@ __device__ __forceinline__ Elem<T> block_exclusive(const Elem<T>& mine, Elem<T>&
 // generic group cumprod
 // ------------------------------------------------------------------------------------------------
 // Tile staging.  A thread owns CH consecutive rows (CH * D words); read straight from global memory, every load
-// instruction of a warp touches 32 different 128-byte lines — r2g measured 79 us for the three launches at L = 1e6 (0.11 of
-// the HBM peak), the LSU wavefront count, not the bytes, set the time.  The tile therefore goes through shared memory:
+// instruction of a warp touches 32 different 128-byte lines, so the LSU wavefront count, not the bytes, sets the time.  The tile therefore goes through shared memory:
 // coalesced 16-byte (or 4/8-byte, when the tile is not 16-byte aligned) global accesses, and each thread's CH * D words sit
 // at stride CH * D + 1 words — odd, so the per-thread reads and writes are bank-conflict free.
 template <typename T, int D, int CH> struct TileSmem {
@@ -208,9 +207,8 @@ __global__ void __launch_bounds__(kScanThreads) cumprod_kernel(const T* __restri
 //   1. every tile (kScanThreads x CH rows) multiplies its rows together              -> aggregate of the tile
 //   2. one CTA per sequence scans the tile aggregates (exclusive)                     -> prefix entering each tile
 //   3. every tile scans its rows again starting from that prefix and stores them
-// The rows are read twice, the second time mostly from L2 (a 28 MB sequence stays resident in the 126 MB L2).  A single
-// pass with decoupled look-back was measured first (r2e: 116 us at L = 1e6): with only ~1000 tiles, all resident at once,
-// every tile had to walk back over hundreds of unfinished predecessors — the look-back chain, not the bandwidth, set the
+// The rows are read twice, the second time mostly from L2 (a 28 MB sequence stays resident in the H100's 50 MB L2).  A
+// single pass with decoupled look-back was slower: with only ~1000 tiles, all resident at once, every tile had to walk back over hundreds of unfinished predecessors — the look-back chain, not the bandwidth, set the
 // time.  Workspace (caller-owned, no initialisation needed): aggregates (tiles x 8) and prefixes (tiles x 8).
 // ------------------------------------------------------------------------------------------------
 // tile aggregates / prefixes live in 8-number slots (the widest group layout) of a 16-byte aligned workspace: moved as
@@ -260,8 +258,8 @@ __global__ void __launch_bounds__(kScanThreads) cumprod_tile_reduce_kernel(const
   if (threadIdx.x == 0) store_agg(agg + gid * 8, total);
 }
 // exclusive scan of the nt tile aggregates of one sequence: one CTA of kPrefixThreads per sequence, one aggregate per
-// thread and round (carry across rounds), two levels of warp-shuffle scans.  r2h ncu: the 128-thread version needed 8
-// rounds of a block scan for the 977 tiles of L = 1e6 and took 17.9 us — longer than either pass over the rows.
+// thread and round (carry across rounds), two levels of warp-shuffle scans (a 128-thread version needs 8 rounds of a block
+// scan for the 977 tiles of L = 1e6).
 constexpr int kPrefixThreads = 1024;
 template <class G, typename T, bool LEFT>
 __global__ void __launch_bounds__(kPrefixThreads) cumprod_tile_prefix_kernel(const T* __restrict__ agg, T* __restrict__ pre, int nt) {
@@ -427,7 +425,7 @@ __device__ __forceinline__ Vpt<T> vpt_block_exclusive(const Vpt<T>& mine, Vpt<T>
 
 // Exp of one gyro increment.  |gyro dt| is ~1e-3 rad for any real IMU, far inside the window where the coefficient series
 // are exact to rounding (theta^2 < small2: remainder < 1e-20), so when every active lane of the warp is inside it the
-// double-precision sincos — ~40 % of the kernel's instructions in round 1 (profiles/r1i_imu_ncu_full_summary.csv) — is not
+// double-precision sincos — the bulk of the general path's instructions — is not
 // executed at all; any lane outside takes the general path for the whole warp (same values as so3_exp(phi, rot_coef(phi))
 // to rounding).
 template <typename T> __device__ __forceinline__ Q4<T> so3_exp_imu(const V3<T>& phi) {
@@ -718,9 +716,8 @@ SCAN_ABI(Sim3, Sim3g)
 
 // ------------------------------------------------------------------------------------------------
 // Predict-only integration with the samples STAGED through shared memory by 1-D TMA bulk copies (tma.cuh).
-// ncu of imu_integrate_kernel (profiles/r1i): 124 registers -> 16 warps per SM, and half of the stall cycles are long-
-// scoreboard waits on the tile's own loads plus LSU back-pressure from 3-word strided stores — the next tile cannot start
-// loading before this one has been scanned.  Here thread 0 queues the bulk loads of tile i+2 while the CTA scans tile i
+// imu_integrate_kernel needs ~124 registers -> 16 warps per SM, and it waits on the tile's own loads plus LSU back-pressure
+// from 3-word strided stores — the next tile cannot start loading before this one has been scanned.  Here thread 0 queues the bulk loads of tile i+2 while the CTA scans tile i
 // out of shared memory, and the results leave through one bulk store per output array, so the LSU only sees shared memory.
 // Same arithmetic, same order of operations as imu_integrate_kernel (results are bit-identical).
 // Preconditions (checked by the launcher, which otherwise uses imu_integrate_kernel): no per-sample `rot`, no integrate
@@ -875,9 +872,8 @@ static int imu_tma_launch(const T* dt, const T* gyro, const T* acc, const T* ini
 }
 
 // Samples per thread (CH) trades scan overhead (amortised over CH) against coalescing (a thread's CH consecutive
-// samples make every warp access CH-strided).  Measured on B200 at 1e3 x 1e4 samples (tools/ab_imu.py): fp64 predict-only
-// 0.61 ms at CH=2 vs 0.72 (CH=1) / 0.74 (CH=4); fp64 with the six integrate outputs 0.74 ms at CH=1 vs 0.79 / 1.14;
-// fp32 predict-only 0.29 ms at CH=2 vs 0.48 (CH=4) / 0.60 (CH=8).  B200POSE_IMU_CH overrides for A/B runs.
+// samples make every warp access CH-strided).  tools/ab_imu.py compares the choices at 1e3 x 1e4 samples;
+// B200POSE_IMU_CH overrides for A/B runs.
 template <typename T, int CH>
 static void imu_launch(const T* dt, const T* gyro, const T* acc, const T* rot, const T* init_rot, long long init_stride,
                        const T* g, T* a, T* Dp, T* Dv, T* Dr, T* Dt, T* w, const T* init_pos, const T* init_vel,

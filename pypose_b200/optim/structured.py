@@ -22,6 +22,7 @@ import torch
 from .. import _C
 from ..lietensor import lietensor as _lt
 from ..lietensor.lietensor import LieTensor, Parameter, SE3_type
+from ..lietensor.scan import _sms
 from . import _fused  # noqa: F401  (registers the ops)
 from . import _lmstep
 
@@ -512,7 +513,8 @@ class BAProblem(_Problem):
         self.cseg = torch.zeros(C + 1, dtype=torch.int32, device=self.pl.device)
         self.cseg[1:] = torch.cumsum(torch.bincount(self.cl, minlength=C), 0).to(torch.int32)
         tpi = 128 if m >= 192 * C else 32
-        want = 148 * 8 * (128 // tpi)                      # items that fill the SMs
+        sms = _sms(self.pl.device) if self.pl.is_cuda else 132     # the geometry only steers the device kernels
+        want = sms * 8 * (128 // tpi)                      # items that fill the SMs
         split = max(1, min(want // max(C, 1), (m // max(C, 1)) // (8 * tpi))) if C < want else 1
         self.geom = (self.cseg, int(split), int(tpi), self.ppos, self.cidx_p, self.pptr, self.pix[self.padj].contiguous())
         self.tol, self.maxiter = tol, maxiter

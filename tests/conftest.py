@@ -1,6 +1,6 @@
 """pytest configuration.
 
-* registers the `gpu` marker (tests that need a real B200);
+* registers the `gpu` marker (tests that need a real H100);
 * gives the `b200pose::*` torch ops a **test-only CPU kernel backed by the oracle**, so the
   host-side logic (LieTensor dispatch, autograd/vmap registrations, LM control flow, gloo
   sharding) can be exercised without a GPU.  The shipped package registers CUDA kernels only —
@@ -20,7 +20,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

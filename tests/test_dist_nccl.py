@@ -23,7 +23,7 @@ def _free_port():
 @pytest.mark.gpu
 def test_sharded_lm_two_gpus_matches_reference(tmp_path, golden_lm):
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs two GPUs")
     out = str(tmp_path / "nccl.npz")
     port = str(_free_port())
     procs = []

@@ -16,8 +16,8 @@ from pypose_b200._optable import GROUPS
 
 pytestmark = pytest.mark.gpu
 OPS = all_ops()
-# fp32: north_star's per-op bound.  Measured maxima on B200 over the random + golden inputs of every op
-# (profiles/r2y_per_op_error_maxima.log): fp32 3.2e-7, fp64 1.1e-13.
+# fp32: north_star's per-op bound.  Measured maxima on H100 over the random + golden inputs of every op:
+# fp32 3.2e-7, fp64 1.1e-13.
 TOL = {torch.float64: 1e-12, torch.float32: 1e-6}
 
 
@@ -112,9 +112,8 @@ def test_full_size_roundtrip_and_properties(grp):
 
     Round-trip tolerance, relative to (1 + |x|), angles U(1e-6, pi - 0.01), |tau| ~ N(0,1):
       fp64: max <= 1e-12.
-      fp32, rows with theta <= pi - 0.05: 99.99 % of the rows <= 1e-6 and max <= 2e-6 (measured on B200, SE3: max
-      1.6e-6 over 987 244 rows, r2e); rows in (pi - 0.05, pi - 0.01] are reported separately and bounded by 4e-6
-      (measured 1.5e-6).  What exceeds 1e-6 is the fp32 quantisation of the materialised group element X (6e-8 relative
+      fp32, rows with theta <= pi - 0.05: 99.99 % of the rows <= 1e-6 and max <= 2e-6; rows in (pi - 0.05, pi - 0.01]
+      are reported separately and bounded by 4e-6.  What exceeds 1e-6 is the fp32 quantisation of the materialised group element X (6e-8 relative
       on q and t, |t| up to ~4, amplified by Jl^-1(phi)); it is a property of storing X in fp32, not of the kernels (the
       same inputs give 3e-15 in fp64).  north_star's 1e-6 is therefore met at the 99.99th percentile, not at the max."""
     alg, D, K = GROUPS[grp]

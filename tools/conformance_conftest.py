@@ -1,8 +1,9 @@
 """conftest used by tools/run_reference_tests.sh: aliases `pypose` to pypose_b200 (CPU, oracle-backed test kernels)."""
 import importlib
+import os
 import sys
 
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, os.environ['PYPOSE_B200_ROOT'])
 import tests.conftest  # noqa: F401,E402
 import pypose_b200  # noqa: E402
 
