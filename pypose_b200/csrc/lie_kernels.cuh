@@ -4,12 +4,16 @@
 // 16-byte multiples, so a per-thread vector load would be misaligned; instead each CTA owns a
 // contiguous chunk of elements and moves it tile-by-tile:
 //
-//   HBM --(16 B coalesced, streaming hint)--> smem tile --(row gather)--> registers
-//        --(lie_math.cuh)--> registers --(row scatter)--> smem tile --(16 B coalesced)--> HBM
+//   global --(16 B coalesced / bulk copy, L2 evict-first)--> smem tile --(row gather)--> registers
+//        --(lie_math.cuh)--> registers --(row scatter)--> smem tile --(16 B coalesced / bulk copy)--> global
 //
-// so every DRAM sector is touched exactly once (algorithmic bytes == DRAM traffic).  The grid is a
-// multiple of the SM count: each CTA gets the same number of elements (chunk), so there is no tail
-// wave.  One element per thread per tile; EPT tiles are batched per barrier to raise bytes in flight.
+// so every input byte is read once and every output byte written once (algorithmic bytes == L2 traffic).
+// L2 policy: an op's input is usually dead after the op, its output is what the next op reads (Exp then
+// Log).  Inputs are therefore read evict-first and outputs stored with normal priority, so the outputs
+// of one launch are still in the 50 MB L2 when the next launch reads them, instead of having been pushed
+// out by the inputs.  The grid is a multiple of the SM count: each CTA gets the same number of elements
+// (chunk), so there is no tail wave.  One element per thread per tile; EPT tiles are batched per barrier
+// to raise bytes in flight.
 #pragma once
 #include "b200pose.h"   // every definition is checked against the generated declaration
 #include <cuda_runtime.h>
@@ -48,8 +52,8 @@ __device__ __forceinline__ void tile_store(T* __restrict__ g, const T* __restric
   float4* g4 = reinterpret_cast<float4*>(g);
   const float4* s4 = reinterpret_cast<const float4*>(s);
 #pragma unroll 4
-  for (int k = threadIdx.x; k < nvec; k += kThreads) __stcs(g4 + k, s4[k]);
-  for (int k = nvec * WPV + threadIdx.x; k < nwords; k += kThreads) __stcs(g + k, s[k]);
+  for (int k = threadIdx.x; k < nvec; k += kThreads) g4[k] = s4[k];
+  for (int k = nvec * WPV + threadIdx.x; k < nwords; k += kThreads) g[k] = s[k];
 }
 
 template <int D, typename T> __device__ __forceinline__ void row_get(const T* __restrict__ s, int row, T (&r)[D]) {
@@ -153,6 +157,7 @@ __global__ void __launch_bounds__(THREADS) stream_kernel_tma(StreamParams<typena
 
   const int last_cnt = ntiles ? (int)(end - begin - (long long)(ntiles - 1) * TILE) : 0;
 
+  const uint64_t in_policy = l2_policy_evict_first();   // inputs are read once: let them leave L2 first
   auto issue_load = [&](int t, int s) {   // thread 0 only: tile t -> stage s
     const long long base = begin + (long long)t * TILE;
     const int cnt = (t == ntiles - 1) ? last_cnt : TILE;
@@ -160,10 +165,12 @@ __global__ void __launch_bounds__(THREADS) stream_kernel_tma(StreamParams<typena
     const uint32_t b0 = cnt * Op::DI0 * sizeof(T), b1 = Op::NIN > 1 ? cnt * Op::DI1 * sizeof(T) : 0,
                    b2 = Op::NIN > 2 ? cnt * Op::DI2 * sizeof(T) : 0;
     mbar_expect_tx(&full[s], b0 + b1 + b2);
-    bulk_g2s(dst, p.in[0] + base * Op::DI0, b0, &full[s]);
-    if (Op::NIN > 1) bulk_g2s(dst + TILE * Op::DI0, p.in[Op::NIN > 1 ? 1 : 0] + base * Op::DI1, b1, &full[s]);
+    bulk_g2s_hint(dst, p.in[0] + base * Op::DI0, b0, &full[s], in_policy);
+    if (Op::NIN > 1)
+      bulk_g2s_hint(dst + TILE * Op::DI0, p.in[Op::NIN > 1 ? 1 : 0] + base * Op::DI1, b1, &full[s], in_policy);
     if (Op::NIN > 2)
-      bulk_g2s(dst + TILE * (Op::DI0 + Op::DI1), p.in[Op::NIN > 2 ? 2 : 0] + base * Op::DI2, b2, &full[s]);
+      bulk_g2s_hint(dst + TILE * (Op::DI0 + Op::DI1), p.in[Op::NIN > 2 ? 2 : 0] + base * Op::DI2, b2, &full[s],
+                    in_policy);
   };
 
   if (tid == 0) {

@@ -32,6 +32,18 @@ __device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, uint3
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
                ::"l"(gdst), "r"(smem_u32(smem_src)), "r"(bytes) : "memory");
 }
+// L2 cache policy (createpolicy) for the .L2::cache_hint form below: build it once per thread, pass it to every copy.
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+// bulk_g2s with an L2 eviction priority for the lines it reads
+__device__ __forceinline__ void bulk_g2s_hint(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar,
+                                              uint64_t policy) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+               ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(policy) : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");

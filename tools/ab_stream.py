@@ -1,5 +1,11 @@
 """Dev tool: time individual C-ABI Lie kernels on a ring of buffers (CUDA graph, events).
-usage: python tools/ab_stream.py [sym ...]   env: B200POSE_STREAM, B200POSE_CTAS_PER_SM"""
+usage: python tools/ab_stream.py [sym ...]   env: B200POSE_STREAM, B200POSE_CTAS_PER_SM
+       python tools/ab_stream.py --chain     bench.py's step with Log's input warm vs cold in L2
+
+--chain times, on bench.py's ring of 8 batches of 1e6 fp32 elements, Exp(slot j) -> Log(slot j) (the benchmark's
+step: Log reads the SE3 batch Exp has just written) and Exp(slot j) -> Log(slot j+4) (same kernels and bytes, but Log's
+input was written four steps, 416 MB of traffic, earlier and is no longer in L2).  cold - chained is what L2 reuse
+between the two launches saves."""
 import ctypes, os, sys, json
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -7,41 +13,85 @@ from pypose_b200 import _C
 from pypose_b200._optable import lie_symbols
 
 N = int(os.environ.get("AB_N", 1_000_000))
-SYMS = sys.argv[1:] or ["b200_se3_exp_fwd_f32", "b200_SE3_log_fwd_f32"]
-TAB = {s: (ct, ins, outs) for s, ct, ins, outs, _ in lie_symbols()}
 dev = torch.device("cuda")
-res = {}
-for sym in SYMS:
-    ct, ins, outs = TAB[sym]
-    dt = torch.float32 if ct == "float" else torch.float64
-    per = sum(w for _, w in ins + outs) * N * (4 if ct == "float" else 8)
-    ring = max(2, int(600e6 // per) + 1)
-    bufs = []
-    for _ in range(ring):
-        i_t = [torch.randn(N, w, dtype=dt, device=dev) * 0.5 for _, w in ins]
-        o_t = [torch.empty(N, w, dtype=dt, device=dev) for _, w in outs]
-        bufs.append((i_t, o_t))
-    f = _C.fn(sym)
+
+
+def graph_of(calls):
+    """warm the calls up once, then capture them into one CUDA graph on a side stream"""
     side = torch.cuda.Stream()
-    def call(j, sp):
-        i_t, o_t = bufs[j]
-        rc = f(*[ctypes.c_void_p(t.data_ptr()) for t in i_t + o_t], N, sp)
-        assert rc == 0, rc
     with torch.cuda.stream(side):
         sp = ctypes.c_void_p(side.cuda_stream)
-        for j in range(ring): call(j, sp)
+        for c in calls: c(sp)
         side.synchronize()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, stream=side):
             spc = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-            for j in range(ring): call(j, spc)
+            for c in calls: c(spc)
     torch.cuda.synchronize()
     g.replay(); torch.cuda.synchronize()
-    trips = max(1, 4000 // ring)
+    return g
+
+
+def us_per_call(g, calls_per_replay, trips):
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
     for _ in range(trips): g.replay()
     b.record(); torch.cuda.synchronize()
-    us = a.elapsed_time(b) * 1e3 / (trips * ring)
-    res[sym] = {"us": round(us, 2), "GBs": round(per / us / 1e3, 1)}
-print(json.dumps({"impl": os.environ.get("B200POSE_STREAM", "v2"), "ctas": os.environ.get("B200POSE_CTAS_PER_SM", "max"), "n": N, **res}))
+    return a.elapsed_time(b) * 1e3 / (trips * calls_per_replay)
+
+
+def run_syms(syms):
+    tab = {s: (ct, ins, outs) for s, ct, ins, outs, _ in lie_symbols()}
+    res = {}
+    for sym in syms:
+        ct, ins, outs = tab[sym]
+        dt = torch.float32 if ct == "float" else torch.float64
+        per = sum(w for _, w in ins + outs) * N * (4 if ct == "float" else 8)
+        ring = max(2, int(600e6 // per) + 1)
+        f = _C.fn(sym)
+        bufs = [([torch.randn(N, w, dtype=dt, device=dev) * 0.5 for _, w in ins],
+                 [torch.empty(N, w, dtype=dt, device=dev) for _, w in outs]) for _ in range(ring)]
+
+        def call(j):
+            def c(sp):
+                i_t, o_t = bufs[j]
+                rc = f(*[ctypes.c_void_p(t.data_ptr()) for t in i_t + o_t], N, sp)
+                assert rc == 0, rc
+            return c
+        g = graph_of([call(j) for j in range(ring)])
+        us = us_per_call(g, ring, max(1, 4000 // ring))
+        res[sym] = {"us": round(us, 2), "GBs": round(per / us / 1e3, 1)}
+    return res
+
+
+def run_chain(regions=5, steps=4000):
+    ring = 8                                     # as bench.py: 8 x 76 MB of distinct buffers
+    xs = [torch.randn(N, 6, device=dev) * 0.5 for _ in range(ring)]
+    Xs = [torch.empty(N, 7, device=dev) for _ in range(ring)]
+    ys = [torch.empty(N, 6, device=dev) for _ in range(ring)]
+    f_exp, f_log = _C.fn("b200_se3_exp_fwd_f32"), _C.fn("b200_SE3_log_fwd_f32")
+    ptr = lambda t: ctypes.c_void_p(t.data_ptr())
+
+    def step(j, k):                              # Exp into slot j, then Log of slot k
+        def c(sp):
+            _C.check(f_exp(ptr(xs[j]), ptr(Xs[j]), N, sp), "exp")
+            _C.check(f_log(ptr(Xs[k]), ptr(ys[k]), N, sp), "log")
+        return c
+    g_chain = graph_of([step(j, j) for j in range(ring)])
+    g_cold = graph_of([step(j, (j + 4) % ring) for j in range(ring)])
+    trips = max(1, steps // ring)
+    chain, cold = [], []
+    for _ in range(regions):                     # alternate the two so drifting clocks hit both alike
+        chain.append(us_per_call(g_chain, ring, trips))
+        cold.append(us_per_call(g_cold, ring, trips))
+    med = lambda v: sorted(v)[len(v) // 2]
+    return {"chained_us": round(med(chain), 2), "cold_us": round(med(cold), 2),
+            "l2_saving_us": round(med(cold) - med(chain), 2),
+            "chained_all": [round(v, 2) for v in chain], "cold_all": [round(v, 2) for v in cold]}
+
+
+if __name__ == "__main__":
+    args = sys.argv[1:]
+    res = run_chain() if args == ["--chain"] else run_syms(args or ["b200_se3_exp_fwd_f32", "b200_SE3_log_fwd_f32"])
+    print(json.dumps({"impl": os.environ.get("B200POSE_STREAM", "v2"), "ctas": os.environ.get("B200POSE_CTAS_PER_SM", "max"),
+                      "n": N, **res}))
