@@ -144,8 +144,9 @@ __global__ void __launch_bounds__(THREADS) stream_kernel_tma(StreamParams<typena
   const int ntiles = begin < end ? (int)((end - begin + TILE - 1) / TILE) : 0;
   const int tid = threadIdx.x;
 
-  // Programmatic dependent launch: let the next kernel in the stream start its launch/prologue now, and
-  // hold our own first global access until the previous kernel has completed and flushed.
+  // Programmatic dependent launch: let the next kernel in the stream start its launch/prologue now (its CTAs fit
+  // beside ours, see launch_stream_tma), and hold our own first global access until the previous kernel has
+  // completed and flushed.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (tid == 0) {
 #pragma unroll
@@ -272,7 +273,8 @@ int launch_stream_ept(const typename Op::T* const* in, typename Op::T* const* ou
   return (int)cudaGetLastError();
 }
 
-// B200POSE_STREAM=v1 forces the plain-load shell (A/B measurements); B200POSE_CTAS_PER_SM caps residency.
+// B200POSE_STREAM=v1 forces the plain-load shell (A/B measurements); B200POSE_CTAS_PER_SM sets the TMA shell's
+// resident CTAs per SM (capped at its occupancy) in place of the default half.
 inline int stream_impl_v1() {
   static int v = -1;
   if (v < 0) { const char* e = getenv("B200POSE_STREAM"); v = (e && e[0] == 'v' && e[1] == '1') ? 1 : 0; }
@@ -283,9 +285,10 @@ inline int stream_pdl() {
   if (v < 0) { const char* e = getenv("B200POSE_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
   return v;
 }
+// 0 = not set: the TMA shell then takes half its occupancy (see launch_stream_tma)
 inline int stream_max_ctas_per_sm() {
   static int v = -1;
-  if (v < 0) { const char* e = getenv("B200POSE_CTAS_PER_SM"); v = e ? atoi(e) : 8; if (v < 1) v = 8; }
+  if (v < 0) { const char* e = getenv("B200POSE_CTAS_PER_SM"); v = e ? atoi(e) : 0; if (v < 0) v = 0; }
   return v;
 }
 
@@ -298,9 +301,14 @@ int launch_stream_tma(const typename Op::T* const* in, typename Op::T* const* ou
   int& occ = occ_dev[current_device_slot()];
   if (occ == 0) {
     if (L::BYTES > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::BYTES);
+    // the largest shared-memory split, so that the SM is not configured for one grid's needs alone
+    cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, L::BYTES);
+    // Half the SM per launch: the CTAs of the next PDL launch in the stream are resident beside this grid while it
+    // runs, and start the moment it completes.  The Exp -> Log step measured 1.1 us faster so (DESIGN §3.1, §6).
+    const int cap = stream_max_ctas_per_sm();
+    occ = cap ? (occ < cap ? occ : cap) : occ / 2;
     if (occ < 1) occ = 1;
-    if (occ > stream_max_ctas_per_sm()) occ = stream_max_ctas_per_sm();
   }
   StreamParams<T, Op::NIN, Op::NOUT> p;
   for (int i = 0; i < Op::NIN; ++i) p.in[i] = in[i];

@@ -1,6 +1,7 @@
 """Dev tool: time individual C-ABI Lie kernels on a ring of buffers (CUDA graph, events).
-usage: python tools/ab_stream.py [sym ...]   env: B200POSE_STREAM, B200POSE_CTAS_PER_SM
+usage: python tools/ab_stream.py [sym ...]   env: B200POSE_STREAM, B200POSE_CTAS_PER_SM, B200POSE_PDL
        python tools/ab_stream.py --chain     bench.py's step with Log's input warm vs cold in L2
+       python tools/ab_stream.py --boundary  cost of one launch boundary (Exp and Log, 8 x N rows in 1 vs 8 launches)
 
 --chain times, on bench.py's ring of 8 batches of 1e6 fp32 elements, Exp(slot j) -> Log(slot j) (the benchmark's
 step: Log reads the SE3 batch Exp has just written) and Exp(slot j) -> Log(slot j+4) (same kernels and bytes, but Log's
@@ -90,8 +91,40 @@ def run_chain(regions=5, steps=4000):
             "chained_all": [round(v, 2) for v in chain], "cold_all": [round(v, 2) for v in cold]}
 
 
+def run_boundary(parts=8, regions=5, trips=200):
+    """Cost of one launch boundary: the same 8 x N rows moved by one launch and by 8 launches of N rows over the 8
+    slices of the same buffer (one CUDA graph each); (eight - one) / 7 is what each boundary adds."""
+    med = lambda v: sorted(v)[len(v) // 2]
+    res = {}
+    for name, sym, wi, wo in (("exp", "b200_se3_exp_fwd_f32", 6, 7), ("log", "b200_SE3_log_fwd_f32", 7, 6)):
+        f = _C.fn(sym)
+        x = torch.randn(parts * N, 6, device=dev) * 0.5
+        if name == "log":                        # Log of valid SE3 rows
+            X = torch.empty(parts * N, 7, device=dev)
+            _C.check(_C.fn("b200_se3_exp_fwd_f32")(x.data_ptr(), X.data_ptr(), parts * N, None), "exp")
+            x = X
+        y = torch.empty(parts * N, wo, device=dev)
+        call = lambda k, n: (lambda sp: _C.check(f(x.data_ptr() + k * N * wi * 4, y.data_ptr() + k * N * wo * 4, n, sp), sym))
+        g_one = graph_of([call(0, parts * N)])
+        g_many = graph_of([call(k, N) for k in range(parts)])
+        one, many = [], []
+        for _ in range(regions):
+            one.append(us_per_call(g_one, 1, trips))
+            many.append(us_per_call(g_many, 1, trips))
+        res[name] = {"one_launch_us": round(med(one), 2), f"{parts}_launches_us": round(med(many), 2),
+                     "per_boundary_us": round((med(many) - med(one)) / (parts - 1), 3),
+                     "one_all": [round(v, 2) for v in one], "many_all": [round(v, 2) for v in many]}
+        del x, y
+    return res
+
+
 if __name__ == "__main__":
     args = sys.argv[1:]
-    res = run_chain() if args == ["--chain"] else run_syms(args or ["b200_se3_exp_fwd_f32", "b200_SE3_log_fwd_f32"])
-    print(json.dumps({"impl": os.environ.get("B200POSE_STREAM", "v2"), "ctas": os.environ.get("B200POSE_CTAS_PER_SM", "max"),
-                      "n": N, **res}))
+    if args == ["--chain"]:
+        res = run_chain()
+    elif args == ["--boundary"]:
+        res = run_boundary()
+    else:
+        res = run_syms(args or ["b200_se3_exp_fwd_f32", "b200_SE3_log_fwd_f32"])
+    print(json.dumps({"impl": os.environ.get("B200POSE_STREAM", "v2"), "ctas": os.environ.get("B200POSE_CTAS_PER_SM", "half"),
+                      "pdl": os.environ.get("B200POSE_PDL", "1"), "n": N, **res}))
