@@ -8,7 +8,7 @@ import os
 
 import torch
 
-from ._optable import lie_symbols, lm_symbols, scan_symbols
+from ._optable import lie_symbols, lm_symbols, scan_symbols, pcl_symbols
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libb200pose.so")
@@ -43,6 +43,7 @@ def _bind(symbol, n_in, n_out, extra=()):
 _LIE = {s: (ct, ins, outs) for s, ct, ins, outs, _ in lie_symbols()}
 _LM = {s: args for s, args, _ in lm_symbols()}
 _SCAN = {s: args for s, args, _ in scan_symbols()}
+_PCL = {s: args for s, args, _ in pcl_symbols()}
 _CT = {"double": ctypes.c_double, "int": ctypes.c_int, "long long": ctypes.c_longlong}
 
 
@@ -57,10 +58,11 @@ def fn(symbol):
             f.restype = ctypes.c_int
             f.argtypes = [ctypes.c_void_p if "*" in t else _CT[t] for t, _, _ in _LM[symbol]] + \
                 [ctypes.c_longlong, ctypes.c_void_p]
-        elif symbol in _SCAN:
+        elif symbol in _SCAN or symbol in _PCL:
             f = getattr(lib(), symbol)
             f.restype = ctypes.c_int
-            f.argtypes = [ctypes.c_void_p if "*" in t else _CT[t] for t, _, _ in _SCAN[symbol]] + [ctypes.c_void_p]
+            args = _SCAN[symbol] if symbol in _SCAN else _PCL[symbol]
+            f.argtypes = [ctypes.c_void_p if "*" in t else _CT[t] for t, _, _ in args] + [ctypes.c_void_p]
         else:
             raise B200PoseError(f"unknown C-ABI symbol {symbol}")
         _fns[symbol] = f

@@ -443,3 +443,42 @@ def scan_symbols():
     for base, args, cite in SCAN_OPS:
         for sfx, ct in DTYPES.items():
             yield f"{base}_{sfx}", [(t.replace("REAL", ct), n, c) for t, n, c in args], cite
+
+
+# ----------------------------------------------------------------------------------------------
+# point clouds (csrc/knn.cu): k-nearest neighbours and point-to-point ICP.  (symbol base, args, citation); REAL as above.
+# ----------------------------------------------------------------------------------------------
+PCL_OPS = [
+    ("b200_knn",
+     [("const REAL*", "ref", "(B|1,N1,D) query points"), ("long long", "ref_bstride", "elements between batch elements, 0 = broadcast"),
+      ("const REAL*", "nbr", "(B|1,N2,D) neighbour points"), ("long long", "nbr_bstride", "0 = broadcast"),
+      ("REAL*", "values", "(B,N1,k) distances, sorted"), ("long long*", "indices", "(B,N1,k) indices into nbr; ties: lower index first"),
+      ("void*", "ws", "b200_knn_workspace_bytes(B, N1, N2, D, k, sizeof(REAL)) bytes, or NULL when that is 0"),
+      ("long long", "B", ""), ("long long", "N1", ""), ("long long", "N2", ""), ("int", "D", "1..16"),
+      ("int", "k", "1..min(32, N2)"), ("int", "ord", "1, 2 or 0 (= inf)"), ("int", "largest", "1: the k farthest")],
+     "knn: norm of the (..., N1, N2, D) difference tensor + topk, pypose/function/geometry.py:228-313; exact brute force, "
+     "no difference tensor"),
+    ("b200_icp",
+     [("const REAL*", "src", "(B|1,Ns,3) source points"), ("long long", "src_bstride", "0 = broadcast"),
+      ("const REAL*", "tgt", "(B|1,Nt,3) target points"), ("long long", "tgt_bstride", "0 = broadcast"),
+      ("const REAL*", "init", "(B|1,7) initial SE3 or NULL = identity"), ("long long", "init_bstride", "7 or 0"),
+      ("REAL*", "out", "(B,7) SE3 A after the last active iteration"), ("REAL*", "err", "(B) mean nearest distance of the last iteration"),
+      ("REAL*", "last", "(B) the stop rule's previous losses"),
+      ("void*", "ws", "b200_icp_workspace_bytes(B, Ns) bytes: state, A in fp64, per-CTA partial sums"),
+      ("long long", "B", ""), ("long long", "Ns", ""), ("long long", "Nt", ""), ("int", "ord", "1, 2 or 0 (= inf)"),
+      ("long long", "first", "1: initialise A, the stop state and `last`; 0: continue"),
+      ("long long", "iters", "iterations to enqueue (two launches each)"),
+      ("int", "decide", "1: ReduceToBason on the device, iterations after the done flag are no-ops; 0: every iteration runs"),
+      ("long long", "max_steps", ""), ("long long", "patience", ""), ("double", "decreasing", ""), ("double", "tol", ""),
+      ("double*", "host_out", "(8) PINNED host memory: [steps, patience count, continual, .., seq] after the last iteration "
+                              "enqueued, and the call waits for it; NULL: nothing is waited for"),
+      ("long long", "seq", "a number different from the previous call's; appears in host_out[7] when the state is complete")],
+     "ICP.forward, pypose/module/icp.py:73-110 (knn -> mean distance -> svdtf -> apply), with "
+     "ReduceToBason.step, pypose/utils/stepper.py:58-95, as the stop rule"),
+]
+
+
+def pcl_symbols():
+    for base, args, cite in PCL_OPS:
+        for sfx, ct in DTYPES.items():
+            yield f"{base}_{sfx}", [(t.replace("REAL", ct), n, c) for t, n, c in args], cite

@@ -1,0 +1,551 @@
+// knn.cu — batched exact brute-force k-nearest-neighbour search and point-to-point ICP (C-ABI: include/b200pose.h,
+// section "point clouds").  DESIGN.md §3.4.
+//
+// k-NN: one thread owns Q queries and keeps each query's top-k list (distance, index) in registers, sorted, with fully
+// unrolled insertion.  The CTA stages tiles of kTile target points in shared memory with coalesced loads of the
+// contiguous (N2, D) rows (D = 3: padded to 4-wide points, one 16-byte broadcast load per target and thread for fp32) and
+// every staged point is compared with all Q queries of the thread.  Distances come from coordinate differences in the data
+// dtype; ord 2 compares squared distances and takes the root of the k outputs only.  Targets are visited in increasing
+// index order and a candidate must be strictly better to enter a list, so equal distances keep the lower index first.
+// When B * N1 is too small to fill the GPU, the N2 range is split over CTAs and a merge kernel combines the per-split
+// lists in split order (same tie rule): deterministic, no atomics.
+//
+// ICP: one iteration is two launches.  (a) k = 1 matching of A * source against target, A applied on the fly, and per-CTA
+// fp64 partial sums of the matched pairs; (b) one CTA per batch element reduces its partials in a fixed order, solves the
+// Kabsch step in fp64 (icp_math.cuh) and composes A <- T A; the last CTA evaluates the ReduceToBason rule over the batch
+// and sets the done flag that turns later enqueued iterations into no-ops.
+#include <cuda_runtime.h>
+#include <math_constants.h>
+#include <initializer_list>
+#include "icp_math.cuh"
+
+#define B200_EXPORT extern "C" __attribute__((visibility("default")))
+
+namespace b200pose {
+namespace {
+
+constexpr int kKnnThreads = 256;
+constexpr int kTile = 256;                 // target points per shared-memory round
+constexpr int kMaxD = 16;
+constexpr int kUpdThreads = 128;
+constexpr int kSums = 17;                  // sum s(3), sum t(3), sum t s^T (9), sum dist, count
+
+template <typename T> struct alignas(4 * sizeof(T)) Pt4 { T x, y, z, w; };
+
+template <typename T> __device__ __forceinline__ T pos_inf();
+template <> __device__ __forceinline__ float pos_inf<float>() { return CUDART_INF_F; }
+template <> __device__ __forceinline__ double pos_inf<double>() { return CUDART_INF; }
+
+template <bool LARGEST, typename T> __device__ __forceinline__ bool better(T a, T b) { return LARGEST ? a > b : a < b; }
+
+// ord: 1, 2 (squared), 0 = inf
+template <int ORD, typename T> __device__ __forceinline__ T dist3(T ax, T ay, T az, const Pt4<T>& p) {
+  const T dx = ax - p.x, dy = ay - p.y, dz = az - p.z;
+  if (ORD == 2) return fma(dz, dz, fma(dy, dy, dx * dx));
+  if (ORD == 1) return fabs(dx) + fabs(dy) + fabs(dz);
+  return fmax(fabs(dx), fmax(fabs(dy), fabs(dz)));
+}
+template <int ORD, typename T> __device__ __forceinline__ T distn(const T (&q)[kMaxD], const T* p, int D) {
+  T acc = T(0);
+#pragma unroll
+  for (int d = 0; d < kMaxD; ++d)
+    if (d < D) {
+      const T t = q[d] - p[d];
+      acc = ORD == 2 ? fma(t, t, acc) : ORD == 1 ? acc + fabs(t) : fmax(acc, fabs(t));
+    }
+  return acc;
+}
+
+// sorted insertion of (d, j) into a register-resident list; strictly better only (ties keep the earlier entry)
+template <int K, bool LARGEST, typename T>
+__device__ __forceinline__ void topk_insert(T (&v)[K], int (&id)[K], T d, int j) {
+  if (better<LARGEST>(d, v[K - 1])) {
+#pragma unroll
+    for (int i = K - 1; i > 0; --i) {
+      if (better<LARGEST>(d, v[i - 1])) { v[i] = v[i - 1]; id[i] = id[i - 1]; }
+      else if (better<LARGEST>(d, v[i])) { v[i] = d; id[i] = j; }
+    }
+    if (better<LARGEST>(d, v[0])) { v[0] = d; id[0] = j; }
+  }
+}
+
+// Shared-memory tile of target points: D == 3 as padded 4-wide points, otherwise D-strided rows.
+template <typename T, int DV> struct Tile;
+template <typename T> struct Tile<T, 3> { Pt4<T> p[kTile]; };
+template <typename T> struct Tile<T, kMaxD> { T p[kTile * kMaxD]; };
+
+template <typename T, int DV, int NT>
+__device__ __forceinline__ void stage_tile(Tile<T, DV>& tl, const T* __restrict__ P, int j0, int n, int D) {
+  const T* src = P + (long long)j0 * D;
+  for (int e = threadIdx.x; e < n * D; e += NT) {
+    const T v = src[e];
+    if (DV == 3) {
+      const int pt = e / 3, c = e - 3 * pt;
+      reinterpret_cast<T*>(&tl.p[pt])[c] = v;
+    } else {
+      reinterpret_cast<T*>(tl.p)[e] = v;
+    }
+  }
+}
+
+// Q queries of this thread against targets [jb, je): the CTA's core loop.  q: query coordinates (D == 3: q[r][0..2]).
+template <typename T, int DV, int K, int ORD, bool LARGEST, int Q, int NT>
+__device__ __forceinline__ void scan_targets(Tile<T, DV>& tl, const T* __restrict__ P, int jb, int je, int D,
+                                             const T (&q)[Q][kMaxD], T (&v)[Q][K], int (&id)[Q][K]) {
+  for (int j0 = jb; j0 < je; j0 += kTile) {
+    const int n = min(kTile, je - j0);
+    __syncthreads();
+    stage_tile<T, DV, NT>(tl, P, j0, n, D);
+    __syncthreads();
+#pragma unroll 4
+    for (int jj = 0; jj < n; ++jj) {
+      if (DV == 3) {
+        const Pt4<T> p = reinterpret_cast<const Tile<T, 3>&>(tl).p[jj];
+#pragma unroll
+        for (int r = 0; r < Q; ++r) topk_insert<K, LARGEST>(v[r], id[r], dist3<ORD>(q[r][0], q[r][1], q[r][2], p), j0 + jj);
+      } else {
+        const T* p = reinterpret_cast<const T*>(tl.p) + jj * D;
+#pragma unroll
+        for (int r = 0; r < Q; ++r) topk_insert<K, LARGEST>(v[r], id[r], distn<ORD>(q[r], p, D), j0 + jj);
+      }
+    }
+  }
+}
+
+template <int ORD, typename T> __device__ __forceinline__ T finish_dist(T d) { return ORD == 2 ? sqrt(d) : d; }
+
+// grid: nqb query blocks x S splits x B batch elements (flattened in x).  S == 1 writes the results, otherwise the
+// per-split lists (all K entries, ord-2 values still squared) go to pv / pi at ((b S + s) N1 + i) K.
+template <typename T, int DV, int K, int ORD, bool LARGEST, int Q>
+__global__ void __launch_bounds__(kKnnThreads) knn_kernel(const T* __restrict__ ref, long long rbs, const T* __restrict__ nbr,
+                                                          long long nbs, int N1, int N2, int D, int kout, int nqb, int S,
+                                                          int chunk, T* __restrict__ vals, long long* __restrict__ idx,
+                                                          T* __restrict__ pv, int* __restrict__ pi) {
+  __shared__ Tile<T, DV> tl;
+  const int qb = blockIdx.x % nqb, rest = blockIdx.x / nqb, s = rest % S, b = rest / S;
+  const T* R = ref + (long long)b * rbs;
+  const T* P = nbr + (long long)b * nbs;
+  T q[Q][kMaxD];
+  T v[Q][K];
+  int id[Q][K];
+#pragma unroll
+  for (int r = 0; r < Q; ++r) {
+    const int i = min((qb * Q + r) * kKnnThreads + (int)threadIdx.x, N1 - 1);
+#pragma unroll
+    for (int d = 0; d < kMaxD; ++d) q[r][d] = (DV == 3 ? d < 3 : d < D) ? R[(long long)i * D + d] : T(0);
+#pragma unroll
+    for (int c = 0; c < K; ++c) { v[r][c] = LARGEST ? -pos_inf<T>() : pos_inf<T>(); id[r][c] = -1; }
+  }
+  const int jb = s * chunk, je = min(N2, jb + chunk);
+  scan_targets<T, DV, K, ORD, LARGEST, Q, kKnnThreads>(tl, P, jb, je, D, q, v, id);
+#pragma unroll
+  for (int r = 0; r < Q; ++r) {
+    const int i = (qb * Q + r) * kKnnThreads + (int)threadIdx.x;
+    if (i >= N1) continue;
+    if (S == 1) {
+      const long long o = ((long long)b * N1 + i) * kout;
+#pragma unroll
+      for (int c = 0; c < K; ++c)
+        if (c < kout) { vals[o + c] = finish_dist<ORD>(v[r][c]); idx[o + c] = id[r][c]; }
+    } else {
+      const long long o = (((long long)b * S + s) * N1 + i) * K;
+#pragma unroll
+      for (int c = 0; c < K; ++c) { pv[o + c] = v[r][c]; pi[o + c] = id[r][c]; }
+    }
+  }
+}
+
+// one thread per (b, i): the S per-split lists, inserted in split order (= index order), give the exact top-k
+template <typename T, int K, int ORD, bool LARGEST>
+__global__ void __launch_bounds__(kKnnThreads) knn_merge_kernel(const T* __restrict__ pv, const int* __restrict__ pi, int S,
+                                                                long long BN1, int N1, int kout, T* __restrict__ vals,
+                                                                long long* __restrict__ idx) {
+  const long long g = (long long)blockIdx.x * kKnnThreads + threadIdx.x;
+  if (g >= BN1) return;
+  const long long b = g / N1, i = g - b * N1;
+  T v[K];
+  int id[K];
+#pragma unroll
+  for (int c = 0; c < K; ++c) { v[c] = LARGEST ? -pos_inf<T>() : pos_inf<T>(); id[c] = -1; }
+  for (int s = 0; s < S; ++s) {
+    const long long o = ((b * S + s) * N1 + i) * K;
+#pragma unroll
+    for (int c = 0; c < K; ++c) topk_insert<K, LARGEST>(v, id, pv[o + c], pi[o + c]);
+  }
+#pragma unroll
+  for (int c = 0; c < K; ++c)
+    if (c < kout) { vals[g * kout + c] = finish_dist<ORD>(v[c]); idx[g * kout + c] = id[c]; }
+}
+
+int sm_count() {
+  static int cache[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64) dev = 0;
+  if (!cache[dev]) {
+    int n = 0;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    cache[dev] = n > 0 ? n : 132;
+  }
+  return cache[dev];
+}
+
+int kbucket(int k) { return k <= 1 ? 1 : k <= 4 ? 4 : k <= 8 ? 8 : k <= 16 ? 16 : 32; }
+int queries_per_thread(int D, int K) { return D != 3 ? 1 : K == 1 ? 4 : K == 4 ? 2 : 1; }
+
+// Split of the N2 range: enough CTAs for ~4 per SM, each split at least 2048 targets, at most 64 splits.
+struct KnnPlan { int nqb, S, chunk, K; };
+KnnPlan knn_plan(long long B, long long N1, long long N2, int D, int k) {
+  KnnPlan p;
+  p.K = kbucket(k);
+  const long long per = (long long)kKnnThreads * queries_per_thread(D, p.K);
+  p.nqb = (int)((N1 + per - 1) / per);
+  const long long base = B * p.nqb, want = 4LL * sm_count();
+  long long S = 1;
+  if (base > 0 && base < want) {
+    S = (want + base - 1) / base;
+    S = min(S, (N2 + 2047) / 2048);
+    S = max(1LL, min(S, 64LL));
+  }
+  long long chunk = (N2 + S - 1) / S;
+  chunk = (chunk + kTile - 1) / kTile * kTile;
+  p.chunk = (int)max(chunk, (long long)kTile);
+  p.S = (int)((N2 + p.chunk - 1) / p.chunk);
+  if (p.S < 1) p.S = 1;
+  return p;
+}
+
+long long knn_ws_bytes(const KnnPlan& p, long long B, long long N1, int elem) {
+  if (p.S <= 1) return 0;
+  const long long n = (long long)p.S * B * N1 * p.K;
+  return (n * elem + 255) / 256 * 256 + n * 4;
+}
+
+template <typename T> struct KnnArgs {
+  const T* ref; long long rbs; const T* nbr; long long nbs; T* vals; long long* idx; void* ws;
+  long long B, N1, N2; int D, k, ord, largest;
+};
+
+template <typename T, int DV, int K, int ORD, bool LARGEST>
+int launch_knn(const KnnArgs<T>& a, cudaStream_t st) {
+  const KnnPlan p = knn_plan(a.B, a.N1, a.N2, a.D, a.k);
+  T* pv = nullptr;
+  int* pi = nullptr;
+  if (p.S > 1) {
+    const long long n = (long long)p.S * a.B * a.N1 * K;
+    pv = reinterpret_cast<T*>(a.ws);
+    pi = reinterpret_cast<int*>(reinterpret_cast<char*>(a.ws) + (n * (long long)sizeof(T) + 255) / 256 * 256);
+  }
+  const long long grid = (long long)p.nqb * p.S * a.B;
+  constexpr int Q = DV != 3 ? 1 : K == 1 ? 4 : K == 4 ? 2 : 1;
+  knn_kernel<T, DV, K, ORD, LARGEST, Q><<<(unsigned)grid, kKnnThreads, 0, st>>>(
+      a.ref, a.rbs, a.nbr, a.nbs, (int)a.N1, (int)a.N2, a.D, a.k, p.nqb, p.S, p.chunk, a.vals, a.idx, pv, pi);
+  if (p.S > 1) {
+    const long long BN1 = a.B * a.N1;
+    knn_merge_kernel<T, K, ORD, LARGEST><<<(unsigned)((BN1 + kKnnThreads - 1) / kKnnThreads), kKnnThreads, 0, st>>>(
+        pv, pi, p.S, BN1, (int)a.N1, a.k, a.vals, a.idx);
+  }
+  return (int)cudaGetLastError();
+}
+
+template <typename T, int DV, int K, int ORD> int knn_l(const KnnArgs<T>& a, cudaStream_t s) {
+  return a.largest ? launch_knn<T, DV, K, ORD, true>(a, s) : launch_knn<T, DV, K, ORD, false>(a, s);
+}
+template <typename T, int DV, int K> int knn_o(const KnnArgs<T>& a, cudaStream_t s) {
+  return a.ord == 1 ? knn_l<T, DV, K, 1>(a, s) : a.ord == 2 ? knn_l<T, DV, K, 2>(a, s) : knn_l<T, DV, K, 0>(a, s);
+}
+template <typename T, int DV> int knn_k(const KnnArgs<T>& a, cudaStream_t s) {
+  switch (kbucket(a.k)) {
+    case 1: return knn_o<T, DV, 1>(a, s);
+    case 4: return knn_o<T, DV, 4>(a, s);
+    case 8: return knn_o<T, DV, 8>(a, s);
+    case 16: return knn_o<T, DV, 16>(a, s);
+    default: return knn_o<T, DV, 32>(a, s);
+  }
+}
+// Every pointer the kernels dereference must be device (or managed) memory: a host pointer that reached this far (a CPU
+// tensor passed through the C-ABI) is refused here instead of faulting inside a kernel.
+bool device_ptrs(std::initializer_list<const void*> ps) {
+  for (const void* p : ps) {
+    if (!p) continue;
+    cudaPointerAttributes at;
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    if (at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) return false;
+  }
+  return true;
+}
+
+template <typename T> int knn_run(const KnnArgs<T>& a, cudaStream_t s) {
+  if (a.B <= 0 || a.N1 <= 0) return 0;
+  if (!a.ref || !a.nbr || !a.vals || !a.idx || !device_ptrs({a.ref, a.nbr, a.vals, a.idx, a.ws})) return (int)cudaErrorInvalidValue;
+  if (a.k < 1 || a.k > 32 || a.k > a.N2 || a.D < 1 || a.D > kMaxD || (a.ord != 0 && a.ord != 1 && a.ord != 2))
+    return (int)cudaErrorInvalidValue;
+  if (a.N1 > 0x7fffffffLL || a.N2 > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+  return a.D == 3 ? knn_k<T, 3>(a, s) : knn_k<T, kMaxD>(a, s);
+}
+
+// ----------------------------------------------------------------------------------------------------------------------
+// ICP
+// ----------------------------------------------------------------------------------------------------------------------
+// workspace: [st: 8 doubles | ticket: 8 doubles | A: B x 12 doubles | partials: B x nx x 17 doubles]
+// st: [0] steps, [1] patience count, [2] continual (0 = done)
+constexpr int kStWords = 8;
+constexpr int kIcpBig = 256 * 4;           // source points per CTA: 256 threads x 4 queries
+constexpr int kIcpSmall = 128;             // 128 threads x 1 query, when the big CTAs would not fill the GPU
+
+bool icp_small(long long B, long long Ns) { return B * ((Ns + kIcpBig - 1) / kIcpBig) < 2LL * sm_count(); }
+long long icp_nx(long long B, long long Ns) {
+  const long long per = icp_small(B, Ns) ? kIcpSmall : kIcpBig;
+  return (Ns + per - 1) / per;
+}
+
+__device__ __forceinline__ double warp_sum(double x) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
+  return x;
+}
+
+// fixed-order block reduction of kSums values; the totals end up in red[0][*] (visible after the final __syncthreads)
+template <int NT> __device__ __forceinline__ void block_sums(double (&acc)[kSums], double (*red)[kSums]) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < kSums; ++k) acc[k] = warp_sum(acc[k]);
+  if (lane == 0)
+#pragma unroll
+    for (int k = 0; k < kSums; ++k) red[w][k] = acc[k];
+  __syncthreads();
+  if (threadIdx.x < kSums) {
+    double s = 0.0;
+    for (int i = 0; i < NT / 32; ++i) s += red[i][threadIdx.x];
+    red[0][threadIdx.x] = s;          // row 0 is only read again by this thread before the barrier below
+  }
+  __syncthreads();
+}
+
+// (a): k = 1 matching of A source against target and the per-CTA fp64 sums.  grid: nx x B (flattened).
+template <typename T, int ORD, int Q, int NT>
+__global__ void __launch_bounds__(NT) icp_match_kernel(const T* __restrict__ src, long long sbs, const T* __restrict__ tgt,
+                                                       long long tbs, int Ns, int Nt, const double* __restrict__ A,
+                                                       const double* st, double* __restrict__ part, int nx, int decide) {
+  if (decide && st[2] == 0.0) return;
+  __shared__ Tile<T, 3> tl;
+  __shared__ double red[NT / 32][kSums];
+  const int x = blockIdx.x % nx, b = blockIdx.x / nx;
+  const T* S = src + (long long)b * sbs;
+  const T* P = tgt + (long long)b * tbs;
+  T Ra[12];
+#pragma unroll
+  for (int k = 0; k < 12; ++k) Ra[k] = (T)A[b * 12 + k];
+  T q[Q][kMaxD];
+  T v[Q][1];
+  int id[Q][1];
+#pragma unroll
+  for (int r = 0; r < Q; ++r) {
+    const int i = min((x * Q + r) * NT + (int)threadIdx.x, Ns - 1);
+    const T px = S[(long long)i * 3], py = S[(long long)i * 3 + 1], pz = S[(long long)i * 3 + 2];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) q[r][c] = fma(Ra[4 * c], px, fma(Ra[4 * c + 1], py, fma(Ra[4 * c + 2], pz, Ra[4 * c + 3])));
+#pragma unroll
+    for (int d = 3; d < kMaxD; ++d) q[r][d] = T(0);
+    v[r][0] = pos_inf<T>();
+    id[r][0] = 0;
+  }
+  scan_targets<T, 3, 1, ORD, false, Q, NT>(tl, P, 0, Nt, 3, q, v, id);
+  const double c0x = (double)P[0], c0y = (double)P[1], c0z = (double)P[2];
+  double acc[kSums];
+#pragma unroll
+  for (int k = 0; k < kSums; ++k) acc[k] = 0.0;
+#pragma unroll
+  for (int r = 0; r < Q; ++r) {
+    const int i = (x * Q + r) * NT + (int)threadIdx.x;
+    if (i >= Ns) continue;
+    const long long j = id[r][0];
+    const double s[3] = {(double)q[r][0] - c0x, (double)q[r][1] - c0y, (double)q[r][2] - c0z};
+    const double t[3] = {(double)P[j * 3] - c0x, (double)P[j * 3 + 1] - c0y, (double)P[j * 3 + 2] - c0z};
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { acc[c] += s[c]; acc[3 + c] += t[c]; }
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) acc[6 + 3 * a + c] += t[a] * s[c];
+    acc[15] += (double)finish_dist<ORD>(v[r][0]);
+    acc[16] += 1.0;
+  }
+  block_sums<NT>(acc, red);
+  if (threadIdx.x < kSums) part[((long long)b * nx + x) * kSums + threadIdx.x] = red[0][threadIdx.x];
+}
+
+__device__ __forceinline__ void icp_publish(const double* st, double* host_out, double seq) {
+  volatile double* o = host_out;
+  o[0] = st[0]; o[1] = st[1]; o[2] = st[2];
+  __threadfence_system();
+  o[kStWords - 1] = seq;
+}
+
+// (b): per batch element: fixed-order reduction, Kabsch, A <- T A, mean distance, SE3 output; the last CTA decides.
+template <typename T>
+__global__ void __launch_bounds__(kUpdThreads) icp_update_kernel(const T* __restrict__ tgt, long long tbs, double* A,
+                                                                 const double* __restrict__ part, int nx, double* st,
+                                                                 unsigned* ticket, T* last, T* err, T* out, int B,
+                                                                 int decide, R2bCtl ctl, double eps, double* host_out,
+                                                                 double seq, int publish) {
+  if (decide && st[2] == 0.0) {
+    if (publish && host_out && blockIdx.x == 0 && threadIdx.x == 0) icp_publish(st, host_out, seq);
+    return;
+  }
+  __shared__ double red[kUpdThreads / 32][kSums];
+  __shared__ bool is_last;
+  const int b = blockIdx.x;
+  double acc[kSums];
+#pragma unroll
+  for (int k = 0; k < kSums; ++k) acc[k] = 0.0;
+  for (int x = threadIdx.x; x < nx; x += kUpdThreads)
+#pragma unroll
+    for (int k = 0; k < kSums; ++k) acc[k] += part[((long long)b * nx + x) * kSums + k];
+  block_sums<kUpdThreads>(acc, red);
+  if (threadIdx.x == 0) {
+    const T* P = tgt + (long long)b * tbs;
+    const double c0[3] = {(double)P[0], (double)P[1], (double)P[2]};
+    double Ab[12], q[4];
+    for (int k = 0; k < 12; ++k) Ab[k] = A[b * 12 + k];
+    icp_step(red[0], c0, eps, Ab);
+    for (int k = 0; k < 12; ++k) A[b * 12 + k] = Ab[k];
+    err[b] = (T)(red[0][15] / red[0][16]);
+    icp_mat2quat(Ab, q);
+    T* o = out + (long long)b * 7;
+    o[0] = (T)Ab[3]; o[1] = (T)Ab[7]; o[2] = (T)Ab[11];
+    o[3] = (T)q[0]; o[4] = (T)q[1]; o[5] = (T)q[2]; o[6] = (T)q[3];
+  }
+  if (!decide) return;
+  __threadfence();
+  if (threadIdx.x == 0) is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  bool below = true, flat = true;
+  for (int bb = threadIdx.x; bb < B; bb += kUpdThreads) {
+    bool bt, fl;
+    icp_r2b_flags<T>(__ldcg(err + bb), last[bb], ctl, bt, fl);
+    below = below && bt;
+    flat = flat && fl;
+  }
+  below = __syncthreads_and(below);
+  flat = __syncthreads_and(flat);
+  for (int bb = threadIdx.x; bb < B; bb += kUpdThreads) last[bb] = __ldcg(err + bb);
+  if (threadIdx.x == 0) {
+    icp_r2b_update(st, below, flat, ctl);
+    *ticket = 0u;
+    if (publish && host_out) icp_publish(st, host_out, seq);
+  }
+}
+
+template <typename T>
+__global__ void icp_init_kernel(const T* __restrict__ init, long long ibs, double* A, double* st, unsigned* ticket, T* last,
+                                T* out, int B) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b == 0) { st[0] = 0.0; st[1] = 0.0; st[2] = 1.0; *ticket = 0u; }
+  if (b >= B) return;
+  double a[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+  if (init) {
+    const T* p = init + (long long)b * ibs;
+    const double q[4] = {(double)p[3], (double)p[4], (double)p[5], (double)p[6]};
+    icp_quat2mat(q, a);
+    a[3] = (double)p[0]; a[7] = (double)p[1]; a[11] = (double)p[2];
+  }
+  for (int k = 0; k < 12; ++k) A[b * 12 + k] = a[k];
+  last[b] = pos_inf<T>();
+  double q[4];                                     // the result if no iteration runs
+  icp_mat2quat(a, q);
+  T* o = out + (long long)b * 7;
+  o[0] = (T)a[3]; o[1] = (T)a[7]; o[2] = (T)a[11];
+  o[3] = (T)q[0]; o[4] = (T)q[1]; o[5] = (T)q[2]; o[6] = (T)q[3];
+}
+
+template <typename T, int ORD>
+void launch_match(const T* src, long long sbs, const T* tgt, long long tbs, long long B, long long Ns, long long Nt,
+                  const double* A, const double* st, double* part, int nx, int decide, cudaStream_t s) {
+  const unsigned grid = (unsigned)(B * nx);
+  if (icp_small(B, Ns))
+    icp_match_kernel<T, ORD, 1, kIcpSmall><<<grid, kIcpSmall, 0, s>>>(src, sbs, tgt, tbs, (int)Ns, (int)Nt, A, st, part, nx, decide);
+  else
+    icp_match_kernel<T, ORD, 4, 256><<<grid, 256, 0, s>>>(src, sbs, tgt, tbs, (int)Ns, (int)Nt, A, st, part, nx, decide);
+}
+
+int wait_seq(double* host_out, long long seq, cudaStream_t s) {
+  volatile double* flag = host_out + (kStWords - 1);
+  for (long long spin = 0;; ++spin) {
+    if (*flag == (double)seq) return 0;
+    if ((spin & 0xffff) == 0xffff) {           // has the stream died or finished without publishing?
+      const cudaError_t e = cudaStreamQuery(s);
+      if (e == cudaSuccess) return *flag == (double)seq ? 0 : (int)cudaErrorUnknown;
+      if (e != cudaErrorNotReady) return (int)e;
+    }
+  }
+}
+
+template <typename T>
+int icp_run(const T* src, long long sbs, const T* tgt, long long tbs, const T* init, long long ibs, T* out, T* err, T* last,
+            void* ws, long long B, long long Ns, long long Nt, int ord, long long first, long long iters, int decide,
+            long long max_steps, long long patience, double decreasing, double tol, double* host_out, long long seq,
+            cudaStream_t s) {
+  if (B <= 0) return 0;
+  if (!src || !tgt || !out || !err || !last || !ws || !device_ptrs({src, tgt, init, out, err, last, ws}))
+    return (int)cudaErrorInvalidValue;
+  if (Ns <= 0 || Nt <= 0 || Ns > 0x7fffffffLL || Nt > 0x7fffffffLL || (ord != 0 && ord != 1 && ord != 2))
+    return (int)cudaErrorInvalidValue;
+  double* st = reinterpret_cast<double*>(ws);
+  unsigned* ticket = reinterpret_cast<unsigned*>(st + kStWords);
+  double* A = st + 2 * kStWords;
+  double* part = A + B * 12;
+  const int nx = (int)icp_nx(B, Ns);
+  const double eps = sizeof(T) == 4 ? 1e-6 : 1e-12;
+  const R2bCtl ctl{max_steps, patience, decreasing, tol};
+  if (host_out) reinterpret_cast<volatile double*>(host_out)[kStWords - 1] = -1.0;
+  if (first) icp_init_kernel<T><<<(unsigned)((B + 127) / 128), 128, 0, s>>>(init, ibs, A, st, ticket, last, out, (int)B);
+  for (long long it = 0; it < iters; ++it) {
+    if (ord == 2) launch_match<T, 2>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, s);
+    else if (ord == 1) launch_match<T, 1>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, s);
+    else launch_match<T, 0>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, s);
+    icp_update_kernel<T><<<(unsigned)B, kUpdThreads, 0, s>>>(tgt, tbs, A, part, nx, st, ticket, last, err, out, (int)B, decide,
+                                                             ctl, eps, host_out, (double)seq, it == iters - 1);
+  }
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return (int)e;
+  if (!host_out || iters <= 0) return 0;
+  return wait_seq(host_out, seq, s);
+}
+
+}  // namespace
+}  // namespace b200pose
+
+using namespace b200pose;
+
+B200_EXPORT long long b200_knn_workspace_bytes(long long B, long long N1, long long N2, long long D, long long k,
+                                               long long elem_size) {
+  if (B <= 0 || N1 <= 0 || N2 <= 0 || k < 1) return 0;
+  return knn_ws_bytes(knn_plan(B, N1, N2, (int)D, (int)k), B, N1, (int)elem_size);
+}
+
+B200_EXPORT long long b200_icp_workspace_bytes(long long B, long long Ns) {
+  if (B <= 0 || Ns <= 0) return 2 * kStWords * 8;
+  return (2 * kStWords + B * 12 + B * icp_nx(B, Ns) * kSums) * 8;
+}
+
+#define B200_KNN_ENTRIES(CT, SFX)                                                                                          \
+  B200_EXPORT int b200_knn_##SFX(const CT* ref, long long ref_bstride, const CT* nbr, long long nbr_bstride, CT* values,    \
+                                 long long* indices, void* ws, long long B, long long N1, long long N2, int D, int k,      \
+                                 int ord, int largest, void* stream) {                                                     \
+    KnnArgs<CT> a{ref, ref_bstride, nbr, nbr_bstride, values, indices, ws, B, N1, N2, D, k, ord, largest};                 \
+    return knn_run<CT>(a, (cudaStream_t)stream);                                                                           \
+  }                                                                                                                        \
+  B200_EXPORT int b200_icp_##SFX(const CT* src, long long src_bstride, const CT* tgt, long long tgt_bstride,               \
+                                 const CT* init, long long init_bstride, CT* out, CT* err, CT* last, void* ws, long long B, \
+                                 long long Ns, long long Nt, int ord, long long first, long long iters, int decide,        \
+                                 long long max_steps, long long patience, double decreasing, double tol,                   \
+                                 double* host_out, long long seq, void* stream) {                                          \
+    return icp_run<CT>(src, src_bstride, tgt, tgt_bstride, init, init_bstride, out, err, last, ws, B, Ns, Nt, ord, first,  \
+                       iters, decide, max_steps, patience, decreasing, tol, host_out, seq, (cudaStream_t)stream);          \
+  }
+
+B200_KNN_ENTRIES(float, f32)
+B200_KNN_ENTRIES(double, f64)

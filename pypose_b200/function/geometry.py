@@ -1,12 +1,61 @@
-"""Projection / reprojection residual models (reference: pypose/function/geometry.py:7-225).
+"""Projection / reprojection residual models and point-cloud functions (reference: pypose/function/geometry.py).
 
-Only the camera-model functions the LM configs use are in scope (SURVEY.md §2 row 12), plus `svdtf`, which EPnP
-(SURVEY.md §8f.4, module/pnp.py) needs; the other point-cloud utilities (knn, filters) are not part of the hot path.
+The camera-model functions the LM configs use (SURVEY.md §2 row 12), `svdtf`, which EPnP (SURVEY.md §8f.4, module/pnp.py)
+needs, and `knn`, the brute-force nearest-neighbour search behind ICP (csrc/knn.cu, DESIGN.md §3.4).  The point-cloud
+filters are not built.
 """
+import ctypes
+import math
+
 import torch
 
+from .. import _C
 from ..basics import pm
 from .checking import is_lietensor
+
+torch.library.define("b200pose::knn", "(Tensor ref, Tensor nbr, int k, int ord, bool largest) -> (Tensor, Tensor)")
+
+_ORD = {1: 1, 2: 2, math.inf: 0}
+
+
+def _bstride(t):
+    return 0 if t.shape[0] == 1 else t.shape[1] * t.shape[2]
+
+
+@torch.library.impl("b200pose::knn", "CUDA")
+def _knn_cuda(ref, nbr, k, ord, largest):
+    """ref (B|1, N1, D), nbr (B|1, N2, D) contiguous, same dtype -> values (B, N1, k), int64 indices (B, N1, k)."""
+    B, N1, N2, D = max(ref.shape[0], nbr.shape[0]), ref.shape[1], nbr.shape[1], ref.shape[2]
+    vals = torch.empty(B, N1, k, dtype=ref.dtype, device=ref.device)
+    idx = torch.empty(B, N1, k, dtype=torch.int64, device=ref.device)
+    if B * N1 == 0:
+        return vals, idx
+    with torch.cuda.device(ref.device):
+        q = _C.lib().b200_knn_workspace_bytes
+        q.restype, q.argtypes = ctypes.c_longlong, [ctypes.c_longlong] * 6
+        nws = int(q(B, N1, N2, D, k, ref.element_size()))
+        ws = torch.empty(nws, dtype=torch.uint8, device=ref.device) if nws else None
+        sym = f"b200_knn_{_C.suffix(ref.dtype)}"
+        _C.check(_C.fn(sym)(ref.data_ptr(), _bstride(ref), nbr.data_ptr(), _bstride(nbr), vals.data_ptr(), idx.data_ptr(),
+                            ws.data_ptr() if ws is not None else None, B, N1, N2, D, k, ord, int(largest),
+                            _C.stream_ptr(ref.device)), sym)
+    return vals, idx
+
+
+@torch.library.register_fake("b200pose::knn")
+def _knn_fake(ref, nbr, k, ord, largest):
+    B, N1 = max(ref.shape[0], nbr.shape[0]), ref.shape[1]
+    return ref.new_empty(B, N1, k), ref.new_empty(B, N1, k, dtype=torch.int64)
+
+
+def _pc_batch(ref, nbr, B):
+    """(..., N, D) -> (1 | prod(B), N, D) contiguous: an operand with one batch element is broadcast by stride 0."""
+    def flat(t):
+        lead = t.shape[:-2]
+        if math.prod(lead) == 1:
+            return t.reshape(1, *t.shape[-2:]).contiguous()
+        return t.expand(*B, *t.shape[-2:]).reshape(math.prod(B), *t.shape[-2:]).contiguous()
+    return flat(ref), flat(nbr)
 
 
 def cart2homo(coordinates: torch.Tensor):
@@ -59,6 +108,58 @@ def reprojerr(points, pixels, intrinsics, extrinsics=None, reduction='none'):
     if reduction == 'sum':
         return err.sum(dim=-1)
     return err
+
+
+def knn(ref, nbr, k=1, ord=2, dim=-1, largest=False, sorted=True):
+    """The k nearest (or, with `largest`, farthest) points of `nbr` (..., N2, D) for every point of `ref` (..., N1, D)
+    under the `ord`-norm (1, 2 or inf) -> `torch.return_types.topk(values (..., N1, k), indices (..., N1, k))`, as the
+    reference (geometry.py:228-313) computes with a (..., N1, N2, D) difference tensor and `topk`.
+
+    Exact brute force on the GPU (csrc/knn.cu) without that tensor: D <= 16, k <= 32, batch dimensions broadcast.  The
+    result is always sorted, and equal distances list the lower index first, so indices are deterministic; `sorted=False`
+    is accepted and returns the same.  `values` is differentiable with respect to `ref` and `nbr`: when either requires
+    grad the values are recomputed with torch ops from the selected neighbours (the selection itself has no gradient).
+
+    Coordinates must be finite.  A candidate enters a list only if its distance compares strictly better, so a NaN
+    distance never does: a query with NaN coordinates, or with fewer than k targets at a non-NaN distance, gets index -1
+    and value inf (-inf with `largest`) in the slots left empty, where `torch.topk` would rank NaN as the largest value."""
+    if not (isinstance(ref, torch.Tensor) and isinstance(nbr, torch.Tensor)):
+        raise TypeError("knn: ref and nbr must be tensors")
+    if not ref.is_cuda or not nbr.is_cuda:
+        raise NotImplementedError(f"knn: expected CUDA tensors (no CPU path), got {ref.device} / {nbr.device}")
+    if ref.device != nbr.device or ref.dtype != nbr.dtype:
+        raise ValueError(f"knn: ref and nbr must share device and dtype, got {ref.device}/{ref.dtype} and {nbr.device}/{nbr.dtype}")
+    _C.suffix(ref.dtype)
+    if ref.dim() < 2 or nbr.dim() < 2:
+        raise ValueError("knn: ref and nbr must have shape (..., N, D)")
+    if dim not in (-1, ref.dim() - 1) or (dim == ref.dim() - 1 and ref.dim() != nbr.dim()):
+        raise ValueError(f"knn: only the last dimension can hold the coordinates, got dim={dim}")
+    if ord not in _ORD:
+        raise ValueError(f"knn: ord must be 1, 2 or inf, got {ord}")
+    D, N1, N2 = ref.shape[-1], ref.shape[-2], nbr.shape[-2]
+    if nbr.shape[-1] != D:
+        raise ValueError(f"knn: ref and nbr have different point dimensions {D} and {nbr.shape[-1]}")
+    if not 1 <= D <= 16:
+        raise ValueError(f"knn: point dimension must be 1..16, got {D}")
+    if not isinstance(k, int) or k < 1 or k > 32:
+        raise ValueError(f"knn: k must be an integer in 1..32, got {k}")
+    if k > N2:
+        raise ValueError(f"knn: k = {k} exceeds the number of neighbours N2 = {N2}")
+    B = torch.broadcast_shapes(ref.shape[:-2], nbr.shape[:-2])
+    if math.prod(B) == 0:
+        vals = ref.new_empty(*B, N1, k)
+        idx = torch.empty(*B, N1, k, dtype=torch.int64, device=ref.device)
+    else:
+        r, n = _pc_batch(ref.detach(), nbr.detach(), B)
+        vals, idx = torch.ops.b200pose.knn(r, n, k, _ORD[ord], bool(largest))
+        vals, idx = vals.view(*B, N1, k), idx.view(*B, N1, k)
+    if torch.is_grad_enabled() and (ref.requires_grad or nbr.requires_grad):
+        nb = nbr.expand(*B, N2, D)
+        found = idx >= 0                  # see the docstring: -1 marks a slot no finite distance filled
+        sel = torch.gather(nb, -2, idx.clamp(min=0).reshape(*B, N1 * k, 1).expand(*B, N1 * k, D)).view(*B, N1, k, D)
+        diff = torch.where(found.unsqueeze(-1), ref.expand(*B, N1, D).unsqueeze(-2) - sel, 0)    # no NaN in the graph
+        vals = torch.where(found, torch.linalg.vector_norm(diff, ord=ord, dim=-1), vals)
+    return torch.return_types.topk((vals, idx))
 
 
 def svdtf(source, target):
