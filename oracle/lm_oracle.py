@@ -131,6 +131,47 @@ def reproj_accum(poses, pts, pix, seg, kind=0, delta=1.0):
     return _triu_pack(A), g, np.array([rho.sum()])
 
 
+def seg_sum(x, seg):
+    """Row sums of x per segment [seg[c], seg[c+1]) of rows sorted by segment: np.add.reduceat over the non-empty
+    segments (reduceat alone returns the next row for an empty one); an empty segment sums to 0."""
+    seg = np.asarray(seg, dtype=np.int64)
+    out = np.zeros((seg.size - 1,) + x.shape[1:], dtype=np.float64)
+    ne = np.flatnonzero(seg[1:] > seg[:-1])
+    if ne.size:
+        out[ne] = np.add.reduceat(x[:seg[-1]], seg[ne], axis=0)
+    return out
+
+
+def reproj_accum_seg(poses, pts, pix, seg, kind=0, delta=1.0):
+    """reproj_accum per camera with a segment reduction over the camera-sorted rows instead of np.add.at (fast at
+    1e6 rows): (C, 21) H, (C, 6) g and the (C,) loss of each camera."""
+    C = poses.shape[0]
+    m = int(seg[-1])
+    cidx = np.repeat(np.arange(C), np.diff(seg))
+    r = reproj_residual(poses, pts[:m], pix[:m], cidx)
+    J = reproj_jac_rows(poses, pts[:m], cidx)
+    rho, w = robust(kind, delta, (r ** 2).sum(-1))
+    iu = np.triu_indices(6)
+    JJ = np.einsum('mka,mkb->mab', J, J)[:, iu[0], iu[1]] * w[:, None]
+    Jr = np.einsum('mka,mk->ma', J, r) * w[:, None]
+    return seg_sum(JJ, seg), seg_sum(Jr, seg), seg_sum(rho, seg)
+
+
+def damped_solve_flagged(A, g, scale, dmin, dmax):
+    """damped_solve per block with a per-block failure flag instead of the exception np.linalg.cholesky raises for the
+    whole batch: (D, predicted, failed), D = 0 and predicted = 0 on the blocks whose damped matrix is not positive
+    definite."""
+    idx = np.arange(A.shape[-1])
+    Ad = A.copy()
+    Ad[..., idx, idx] = np.clip(Ad[..., idx, idx], dmin, dmax) * scale
+    failed = np.linalg.eigvalsh(Ad)[..., 0] <= 0
+    D, pred = np.zeros(g.shape), np.zeros(g.shape[:-1])
+    ok = ~failed
+    if ok.any():
+        D[ok], pred[ok] = damped_solve(A[ok], g[ok], scale, dmin, dmax)
+    return D, pred, failed
+
+
 def solve6_retract(H21, g, P, scale, dmin, dmax):
     D, pred = damped_solve(_triu_unpack(H21), g, scale, dmin, dmax)
     return retract(D, P), D, np.array([pred.sum(), 0.0])
