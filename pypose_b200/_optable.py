@@ -475,6 +475,28 @@ PCL_OPS = [
       ("long long", "seq", "a number different from the previous call's; appears in host_out[7] when the state is complete")],
      "ICP.forward, pypose/module/icp.py:73-110 (knn -> mean distance -> svdtf -> apply), with "
      "ReduceToBason.step, pypose/utils/stepper.py:58-95, as the stop rule"),
+    ("b200_radius_mask",
+     [("const REAL*", "pts", "(N,D) points"), ("long long", "N", ""), ("int", "D", "1..16"),
+      ("double", "thr", "ord 2: largest squared distance kept (a value of REAL); ord 1 / inf: the radius as a REAL"),
+      ("int", "ord", "1, 2 or 0 (= inf)"), ("long long", "need", "keep a point when its count, itself included, is >= need"),
+      ("unsigned char*", "mask_out", "(N) 1 = kept")],
+     "the radius count of nbr_filter / knn_filter, pypose/function/geometry.py:487-489, 652-657; no (N, N) tensor"),
+    ("b200_voxel_sort",
+     [("const REAL*", "pts", "(N,D) points"), ("long long", "N", ""), ("int", "D", ""), ("int", "vdim", "1..min(16, D)"),
+      ("const double*", "bounds_host", "HOST (2 vdim): [min_d, size_d] as values of REAL"),
+      ("const long long*", "plan_host", "HOST (3 vdim + ngroups): [lo_d, group_d, shift_d] per dimension, then the bits "
+                                        "of each key group"),
+      ("int", "ngroups", "key groups, group 0 most significant"),
+      ("void*", "ws", "b200_voxel_workspace_bytes(N) bytes, passed unchanged to b200_voxel_reduce"),
+      ("long long*", "vid", "(N) voxel of every point"), ("long long*", "M", "(1) number of voxels")],
+     "voxel_filter: integer voxel coordinates + torch.unique(dim=-2), pypose/function/geometry.py:579-583"),
+    ("b200_voxel_reduce",
+     [("const REAL*", "pts", "(N,D) the points given to b200_voxel_sort"), ("long long", "N", ""), ("int", "D", ""),
+      ("void*", "ws", "the workspace of b200_voxel_sort"), ("long long", "M", "its voxel count"),
+      ("const double*", "u", "(M) uniforms in [0, 1) to pick one member per voxel, or NULL for centroids"),
+      ("REAL*", "out", "(M,D) centroids when u is NULL"), ("REAL*", "count", "(M) member counts in REAL, or NULL"),
+      ("long long*", "sel", "(M) the picked rows when u is given")],
+     "voxel_filter: index_add_ centroids / the per-voxel random member, pypose/function/geometry.py:584-602"),
 ]
 
 

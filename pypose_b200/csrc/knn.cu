@@ -1,5 +1,5 @@
-// knn.cu — batched exact brute-force k-nearest-neighbour search and point-to-point ICP (C-ABI: include/b200pose.h,
-// section "point clouds").  DESIGN.md §3.4.
+// knn.cu — batched exact brute-force k-nearest-neighbour search, point-to-point ICP and the radius mask of the
+// point-cloud filters (C-ABI: include/b200pose.h, section "point clouds").  DESIGN.md §3.4, §3.5.
 //
 // k-NN: one thread owns Q queries and keeps each query's top-k list (distance, index) in registers, sorted, with fully
 // unrolled insertion.  The CTA stages tiles of kTile target points in shared memory with coalesced loads of the
@@ -285,6 +285,97 @@ template <typename T> int knn_run(const KnnArgs<T>& a, cudaStream_t s) {
 }
 
 // ----------------------------------------------------------------------------------------------------------------------
+// Radius mask (nbr_filter / knn_filter): count the points within `thr` of every point, itself included, and keep it when
+// the count reaches `need`.  Same layout as the k-NN search (Q queries per thread, 256-point tiles in shared memory);
+// ord 2 compares squared distances against the host-computed threshold (DESIGN.md §3.5).  After each tile the CTA stops
+// when every live query already has its count: the mask does not depend on how many tiles were visited.
+// ----------------------------------------------------------------------------------------------------------------------
+template <typename T, int DV, int ORD, int Q>
+__global__ void __launch_bounds__(kKnnThreads) radius_mask_kernel(const T* __restrict__ P, int N, int D, T thr, int need,
+                                                                  unsigned char* __restrict__ mask) {
+  __shared__ Tile<T, DV> tl;
+  T q[Q][kMaxD];
+  int cnt[Q];
+  bool live[Q];
+#pragma unroll
+  for (int r = 0; r < Q; ++r) {
+    const int i0 = (blockIdx.x * Q + r) * kKnnThreads + (int)threadIdx.x;
+    const int i = min(i0, N - 1);
+    live[r] = i0 < N;
+    cnt[r] = 0;
+#pragma unroll
+    for (int d = 0; d < kMaxD; ++d) q[r][d] = (DV == 3 ? d < 3 : d < D) ? P[(long long)i * D + d] : T(0);
+  }
+  for (int j0 = 0; j0 < N; j0 += kTile) {
+    const int n = min(kTile, N - j0);
+    __syncthreads();
+    stage_tile<T, DV, kKnnThreads>(tl, P, j0, n, D);
+    __syncthreads();
+#pragma unroll 4
+    for (int jj = 0; jj < n; ++jj) {
+      if (DV == 3) {
+        const Pt4<T> p = reinterpret_cast<const Tile<T, 3>&>(tl).p[jj];
+#pragma unroll
+        for (int r = 0; r < Q; ++r) cnt[r] += dist3<ORD>(q[r][0], q[r][1], q[r][2], p) <= thr;
+      } else {
+        const T* p = reinterpret_cast<const T*>(tl.p) + jj * D;
+#pragma unroll
+        for (int r = 0; r < Q; ++r) cnt[r] += distn<ORD>(q[r], p, D) <= thr;
+      }
+    }
+    bool done = true;
+#pragma unroll
+    for (int r = 0; r < Q; ++r) done = done && (!live[r] || cnt[r] >= need);
+    if (__syncthreads_and(done)) break;
+  }
+#pragma unroll
+  for (int r = 0; r < Q; ++r) {
+    const int i = (blockIdx.x * Q + r) * kKnnThreads + (int)threadIdx.x;
+    if (i < N) mask[i] = cnt[r] >= need;
+  }
+}
+
+__global__ void fill_bytes_kernel(unsigned char* __restrict__ out, long long n, unsigned char v) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) out[i] = v;
+}
+
+// One query per thread when four per thread would leave SMs idle (fewer than 2 CTAs per SM).
+bool radius_small(long long N) { return (N + 4LL * kKnnThreads - 1) / (4LL * kKnnThreads) < 2LL * sm_count(); }
+
+template <typename T, int DV, int ORD> void launch_radius(const T* P, int N, int D, T thr, int need, unsigned char* mask,
+                                                          cudaStream_t s) {
+  if (DV == 3 && !radius_small(N)) {
+    radius_mask_kernel<T, DV, ORD, 4><<<(unsigned)((N + 4 * kKnnThreads - 1) / (4 * kKnnThreads)), kKnnThreads, 0, s>>>(
+        P, N, D, thr, need, mask);
+  } else {
+    radius_mask_kernel<T, DV, ORD, 1><<<(unsigned)((N + kKnnThreads - 1) / kKnnThreads), kKnnThreads, 0, s>>>(
+        P, N, D, thr, need, mask);
+  }
+}
+
+template <typename T, int DV> void radius_o(const T* P, int N, int D, T thr, int ord, int need, unsigned char* mask,
+                                            cudaStream_t s) {
+  if (ord == 2) launch_radius<T, DV, 2>(P, N, D, thr, need, mask, s);
+  else if (ord == 1) launch_radius<T, DV, 1>(P, N, D, thr, need, mask, s);
+  else launch_radius<T, DV, 0>(P, N, D, thr, need, mask, s);
+}
+
+template <typename T>
+int radius_run(const T* P, long long N, int D, double thr, int ord, long long need, unsigned char* mask, cudaStream_t s) {
+  if (N <= 0) return 0;
+  if (!P || !mask || !device_ptrs({P, mask})) return (int)cudaErrorInvalidValue;
+  if (D < 1 || D > kMaxD || (ord != 0 && ord != 1 && ord != 2) || N > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+  if (need <= 0) {
+    fill_bytes_kernel<<<(unsigned)min((N + 255) / 256, 4096LL), 256, 0, s>>>(mask, N, 1);
+    return (int)cudaGetLastError();
+  }
+  const int nd = (int)min(need, N + 1);       // a count never exceeds N
+  if (D == 3) radius_o<T, 3>(P, (int)N, D, (T)thr, ord, nd, mask, s);
+  else radius_o<T, kMaxD>(P, (int)N, D, (T)thr, ord, nd, mask, s);
+  return (int)cudaGetLastError();
+}
+
+// ----------------------------------------------------------------------------------------------------------------------
 // ICP
 // ----------------------------------------------------------------------------------------------------------------------
 // workspace: [st: 8 doubles | ticket: 8 doubles | A: B x 12 doubles | partials: B x nx x 17 doubles]
@@ -537,6 +628,10 @@ B200_EXPORT long long b200_icp_workspace_bytes(long long B, long long Ns) {
                                  int ord, int largest, void* stream) {                                                     \
     KnnArgs<CT> a{ref, ref_bstride, nbr, nbr_bstride, values, indices, ws, B, N1, N2, D, k, ord, largest};                 \
     return knn_run<CT>(a, (cudaStream_t)stream);                                                                           \
+  }                                                                                                                        \
+  B200_EXPORT int b200_radius_mask_##SFX(const CT* pts, long long N, int D, double thr, int ord, long long need,           \
+                                         unsigned char* mask_out, void* stream) {                                          \
+    return radius_run<CT>(pts, N, D, thr, ord, need, mask_out, (cudaStream_t)stream);                                      \
   }                                                                                                                        \
   B200_EXPORT int b200_icp_##SFX(const CT* src, long long src_bstride, const CT* tgt, long long tgt_bstride,               \
                                  const CT* init, long long init_bstride, CT* out, CT* err, CT* last, void* ws, long long B, \
