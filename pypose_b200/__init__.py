@@ -29,3 +29,4 @@ from .module.loss import geodesic_loss
 from . import optim
 from . import testing
 from . import utils
+from . import metric

@@ -504,3 +504,52 @@ def pcl_symbols():
     for base, args, cite in PCL_OPS:
         for sfx, ct in DTYPES.items():
             yield f"{base}_{sfx}", [(t.replace("REAL", ct), n, c) for t, n, c in args], cite
+
+
+# ----------------------------------------------------------------------------------------------
+# trajectory metrics (csrc/traj.cu): pp.metric.ape / rpe.  (symbol base, args, citation, typed); typed entries come in
+# _f32 / _f64 flavours with REAL as above, the others have one symbol.  Stamps, errors and the Sim3 are fp64.
+# ----------------------------------------------------------------------------------------------
+TRAJ_OPS = [
+    ("b200_traj_match",
+     [("const double*", "s_short", "(n_short) stamps of the shorter trajectory"), ("long long", "n_short", ""),
+      ("const double*", "s_long", "(n_long) stamps of the longer trajectory"), ("long long", "n_long", ""),
+      ("double", "offset", "added to s_long"), ("double", "diff", "a match needs |s_short - (s_long + offset)| < diff"),
+      ("void*", "ws", "b200_traj_workspace_bytes(n_short) bytes"),
+      ("long long*", "idx_short", "(n_short) matched short indices, increasing"), ("long long*", "idx_long", "(n_short) their long indices"),
+      ("long long*", "info", "(3) [matches, s_short not non-decreasing, s_long not non-decreasing]")],
+     "matching_time_indices + the order asserts of StampedSE3, pypose/metric/ape_rpe.py:46-47, 107-139; no (n_short, "
+     "n_long) matrix", False),
+    ("b200_traj_pairs_dist",
+     [("const REAL*", "pose", "SE3 rows"), ("long long", "row_stride", "elements"), ("long long", "col_stride", "elements"),
+      ("const long long*", "idx", "(n) rows of the trajectory"), ("long long", "n", ""),
+      ("const double*", "sim3", "(8) alignment applied to every row, or NULL"), ("double", "delta", "path length"),
+      ("double", "tol", "all: accept when | |D_j - D_i| - delta | <= tol"), ("int", "all", ""),
+      ("void*", "ws", "b200_traj_workspace_bytes(n) bytes"),
+      ("long long*", "src", "(n) all: pair sources; else the walk's indices"), ("long long*", "tgt", "(n) all: pair targets"),
+      ("long long*", "count", "(1) all: pairs; else indices of the walk")],
+     "pairs_by_dist, pypose/metric/ape_rpe.py:100-104, 322-365", True),
+    ("b200_traj_err",
+     [("const REAL*", "rpose", "SE3 rows"), ("long long", "r_row_stride", ""), ("long long", "r_col_stride", ""),
+      ("const REAL*", "epose", "SE3 rows"), ("long long", "e_row_stride", ""), ("long long", "e_col_stride", ""),
+      ("const long long*", "r_a", "(M)"), ("const long long*", "r_b", "(M) RPE, NULL for APE"),
+      ("const long long*", "e_a", "(M)"), ("const long long*", "e_b", "(M) RPE, NULL for APE"),
+      ("const double*", "sim3", "(8) alignment of the estimate, or NULL"), ("long long", "M", "pairs"),
+      ("int", "etype", "0 translation, 1 rotation, 2 pose, 3 radian, 4 degree"), ("double*", "err", "(M)")],
+     "StampedSE3.align + compute_error, pypose/metric/ape_rpe.py:58-66, 240-264, 686-689", True),
+    ("b200_traj_stats",
+     [("const double*", "err", "(M)"), ("long long", "M", ">= 1"),
+      ("int", "mask", "bit 3: median, bit 6: STD (the other statistics are always computed)"),
+      ("void*", "ws", "b200_traj_workspace_bytes(0) bytes"),
+      ("double*", "out", "(7) [Max, Min, Mean, Median, RMSE, SSE, STD] of |err|")],
+     "the statistics of compute_error, pypose/metric/ape_rpe.py:266-288", False),
+]
+
+
+def traj_symbols():
+    for base, args, cite, typed in TRAJ_OPS:
+        if not typed:
+            yield base, args, cite
+            continue
+        for sfx, ct in DTYPES.items():
+            yield f"{base}_{sfx}", [(t.replace("REAL", ct), n, c) for t, n, c in args], cite
