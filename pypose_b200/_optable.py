@@ -553,3 +553,46 @@ def traj_symbols():
             continue
         for sfx, ct in DTYPES.items():
             yield f"{base}_{sfx}", [(t.replace("REAL", ct), n, c) for t, n, c in args], cite
+
+
+# ----------------------------------------------------------------------------------------------
+# LQR (csrc/lqr.cu): batched Riccati solves for affine dynamics and their KKT adjoint.  (symbol base, args, citation);
+# REAL as above.  Operands are contiguous per (problem, step) and read through a batch and a time stride in elements,
+# either of which may be 0; n = ns + nc <= 32.
+# ----------------------------------------------------------------------------------------------
+_LQR_OPERANDS = [
+    ("const REAL*", "Q", "(n,n) per problem and step"), ("long long", "Q_bs", ""), ("long long", "Q_ts", ""),
+    ("const REAL*", "p", "(n)"), ("long long", "p_bs", ""), ("long long", "p_ts", ""),
+    ("const REAL*", "A", "(ns,ns)"), ("long long", "A_bs", ""), ("long long", "A_ts", ""),
+    ("const REAL*", "B", "(ns,nc)"), ("long long", "B_bs", ""), ("long long", "B_ts", ""),
+    ("const REAL*", "c1", "(ns) or NULL = 0"), ("long long", "c1_bs", ""), ("long long", "c1_ts", ""),
+    ("const REAL*", "x_init", "(nb,ns)"), ("const REAL*", "u_traj", "(nc) or NULL = 0"), ("long long", "u_bs", ""),
+    ("long long", "u_ts", ""),
+]
+_LQR_SIZES = [("void*", "ws", ""), ("long long", "nb", ""), ("int", "T", ">= 1"), ("int", "ns", ">= 1"),
+              ("int", "nc", ">= 1, ns + nc <= 32")]
+LQR_OPS = [
+    ("b200_lqr_affine",
+     _LQR_OPERANDS + [("REAL*", "x", "(nb,T+1,ns)"), ("REAL*", "u", "(nb,T,nc)"), ("REAL*", "cost", "(nb), summed in fp64"),
+                      ("REAL*", "x_traj", "(nb,T,ns) the rollout of u_traj"),
+                      ("int*", "status", "(nb) 1 where a Quu is not positive definite")]
+     + [(t, n, "nb*T*nc*(ns+1) elements of REAL" if n == "ws" else c) for t, n, c in _LQR_SIZES],
+     "LQR.forward = lqr_backward + lqr_forward with runsys, pypose/module/lqr.py:306-380 and "
+     "pypose/module/dynamics.py:651-666"),
+    ("b200_lqr_affine_bwd",
+     _LQR_OPERANDS + [("const REAL*", "x", "(nb,T+1,ns) the solution"), ("const REAL*", "u", "(nb,T,nc) the solution"),
+                      ("const REAL*", "gx", "(nb,T+1,ns) or NULL = 0"), ("const REAL*", "gu", "(nb,T,nc) or NULL = 0"),
+                      ("const REAL*", "gcost", "(nb) or NULL = 0"),
+                      ("REAL*", "gQ", "(nb,T|1,n,n) symmetric"), ("int", "gQ_tv", "1: per step, 0: summed over the steps"),
+                      ("REAL*", "gp", "(nb,T|1,n)"), ("int", "gp_tv", ""), ("REAL*", "gA", "(nb,T|1,ns,ns)"),
+                      ("int", "gA_tv", ""), ("REAL*", "gB", "(nb,T|1,ns,nc)"), ("int", "gB_tv", ""),
+                      ("REAL*", "gc1", "(nb,T|1,ns) or NULL"), ("int", "gc1_tv", ""), ("REAL*", "gx_init", "(nb,ns)")]
+     + [(t, n, "nb*T*(nc*(ns+1)+ns+nc) elements of REAL" if n == "ws" else c) for t, n, c in _LQR_SIZES],
+     "autograd through pypose/module/lqr.py:310-380 (KKT adjoint, Amos et al. 2018)"),
+]
+
+
+def lqr_symbols():
+    for base, args, cite in LQR_OPS:
+        for sfx, ct in DTYPES.items():
+            yield f"{base}_{sfx}", [(t.replace("REAL", ct), n, c) for t, n, c in args], cite
