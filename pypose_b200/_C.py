@@ -8,7 +8,7 @@ import os
 
 import torch
 
-from ._optable import lie_symbols, lm_symbols, scan_symbols, pcl_symbols, traj_symbols, lqr_symbols
+from ._optable import lie_symbols, lm_symbols, scan_symbols, pcl_symbols, traj_symbols, lqr_symbols, sparse_symbols
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libb200pose.so")
@@ -46,6 +46,7 @@ _SCAN = {s: args for s, args, _ in scan_symbols()}
 _PCL = {s: args for s, args, _ in pcl_symbols()}
 _TRAJ = {s: args for s, args, _ in traj_symbols()}
 _LQR = {s: args for s, args, _ in lqr_symbols()}
+_SPARSE = {s: args for s, args, _ in sparse_symbols()}
 _CT = {"double": ctypes.c_double, "int": ctypes.c_int, "long long": ctypes.c_longlong}
 
 
@@ -60,10 +61,10 @@ def fn(symbol):
             f.restype = ctypes.c_int
             f.argtypes = [ctypes.c_void_p if "*" in t else _CT[t] for t, _, _ in _LM[symbol]] + \
                 [ctypes.c_longlong, ctypes.c_void_p]
-        elif symbol in _SCAN or symbol in _PCL or symbol in _TRAJ or symbol in _LQR:
+        elif symbol in _SCAN or symbol in _PCL or symbol in _TRAJ or symbol in _LQR or symbol in _SPARSE:
             f = getattr(lib(), symbol)
             f.restype = ctypes.c_int
-            args = next(t[symbol] for t in (_SCAN, _PCL, _TRAJ, _LQR) if symbol in t)
+            args = next(t[symbol] for t in (_SCAN, _PCL, _TRAJ, _LQR, _SPARSE) if symbol in t)
             f.argtypes = [ctypes.c_void_p if "*" in t else _CT[t] for t, _, _ in args] + [ctypes.c_void_p]
         else:
             raise B200PoseError(f"unknown C-ABI symbol {symbol}")

@@ -30,3 +30,5 @@ from . import optim
 from . import testing
 from . import utils
 from . import metric
+from . import sparse
+from .sparse import bsr_bsc_matmul

@@ -596,3 +596,56 @@ def lqr_symbols():
     for base, args, cite in LQR_OPS:
         for sfx, ct in DTYPES.items():
             yield f"{base}_{sfx}", [(t.replace("REAL", ct), n, c) for t, n, c in args], cite
+
+
+# ----------------------------------------------------------------------------------------------
+# block-sparse products (csrc/bsr.cu): pp.bsr_bsc_matmul.  (symbol base, args, citation, typed) as TRAJ_OPS.  A is BSR
+# (sm block rows, sn block columns), B is BSC (sn block rows, sp block columns); indices are int64 on the device.  Values
+# are read through element strides (block, row, column).  A triple is (a << 32) | b: the A and B entries of one block
+# product, ordered by (i, j, k).
+# ----------------------------------------------------------------------------------------------
+_BSR_VALUES = [("const REAL*", "A", "(nnzA,dm,dn) A's values"), ("long long", "a_sb", ""), ("long long", "a_s0", ""),
+               ("long long", "a_s1", ""),
+               ("const REAL*", "B", "(nnzB,dn,dp) B's values"), ("long long", "b_sb", ""), ("long long", "b_s0", ""),
+               ("long long", "b_s1", "")]
+SPARSE_OPS = [
+    ("b200_bsr_count",
+     [("const long long*", "a_crow", "(sm+1)"), ("const long long*", "a_col", "(nnzA)"), ("long long", "sm", ">= 1"),
+      ("long long", "nnzA", ""), ("const long long*", "b_ccol", "(sp+1)"), ("const long long*", "b_row", "(nnzB)"),
+      ("long long", "sp", ">= 1"), ("long long", "nnzB", ""), ("long long", "sn", ">= 1"),
+      ("void*", "ws", "b200_bsr_workspace_bytes(0, sn, nnzA, nnzB, 0) bytes, passed unchanged to b200_bsr_expand"),
+      ("long long*", "info", "(2) [block products T, 1 if an index structure is invalid]")],
+     "bsr_bsc_matmul: the index merge of every (block row, block column) pair, pypose/sparse/ops.py:62-83", False),
+    ("b200_bsr_expand",
+     [("const long long*", "a_col", "(nnzA)"), ("long long", "nnzA", ">= 1"), ("long long", "sm", ""),
+      ("long long", "sp", ""), ("long long", "sn", ""), ("long long", "nnzB", ">= 1"),
+      ("void*", "ws_count", "the workspace of b200_bsr_count"), ("long long", "T", "1 .. 2^31-1, its info[0]"),
+      ("void*", "ws", "b200_bsr_workspace_bytes(1, 0, 0, 0, T) bytes, passed unchanged to b200_bsr_numeric"),
+      ("unsigned long long*", "tri", "(T) triples in (i, j, k) order"), ("int*", "seg", "(T) output block of each triple"),
+      ("long long*", "nnz", "(1) output blocks")],
+     "bsr_bsc_matmul: the output pattern built on the host, pypose/sparse/ops.py:84-98", False),
+    ("b200_bsr_numeric",
+     _BSR_VALUES + [("int", "dm", ""), ("int", "dn", ""), ("int", "dp", ""), ("long long", "sm", ""), ("long long", "sp", ""),
+                    ("long long", "T", ""), ("void*", "ws", "the workspace of b200_bsr_expand"),
+                    ("const unsigned long long*", "tri", "(T)"), ("const int*", "seg", "(T)"), ("long long", "nnz", ">= 1"),
+                    ("long long*", "crow", "(sm+1)"), ("long long*", "col", "(nnz)"),
+                    ("REAL*", "C", "(nnz,dm,dp) contiguous")],
+     "bsr_bsc_matmul: bmm of the gathered blocks + scatter_add_, pypose/sparse/ops.py:86-89", True),
+    ("b200_bsr_grad",
+     _BSR_VALUES + [("const REAL*", "dC", "(nnz,dm,dp) contiguous"), ("int", "dm", ""), ("int", "dn", ""),
+                    ("int", "dp", ""), ("const unsigned long long*", "tri", "(T) of b200_bsr_expand"),
+                    ("const int*", "seg", "(T) of b200_bsr_expand"), ("long long", "T", ""), ("long long", "nnzA", ">= 1"),
+                    ("long long", "nnzB", ">= 1"),
+                    ("void*", "ws", "b200_bsr_workspace_bytes(2, 0, nnzA, nnzB, T) bytes"),
+                    ("REAL*", "dA", "(nnzA,dm,dn) contiguous, or NULL"), ("REAL*", "dB", "(nnzB,dn,dp) contiguous, or NULL")],
+     "autograd of the values of bsr_bsc_matmul (the reference's result carries none)", True),
+]
+
+
+def sparse_symbols():
+    for base, args, cite, typed in SPARSE_OPS:
+        if not typed:
+            yield base, args, cite
+            continue
+        for sfx, ct in DTYPES.items():
+            yield f"{base}_{sfx}", [(t.replace("REAL", ct), n, c) for t, n, c in args], cite
