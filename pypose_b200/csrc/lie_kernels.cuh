@@ -1,8 +1,9 @@
 // lie_kernels.cuh — HBM streaming shell + per-op functors for the LieTensor op family.
 //
 // Data layout in HBM: row-major (N, d) arrays with d in 3..9 words (12..72 B rows).  Rows are not
-// 16-byte multiples, so a per-thread vector load would be misaligned; instead each CTA owns a
-// contiguous chunk of elements and moves it tile-by-tile:
+// 16-byte multiples, so a per-thread vector load would be misaligned; instead each CTA moves whole
+// tiles of 256 rows, dealt round-robin to the CTAs of a persistent grid (CTA b takes tiles b, b + grid,
+// ...), so that everything in flight at one moment lies in one contiguous window that sweeps the arrays once:
 //
 //   global --(16 B coalesced / bulk copy, L2 evict-first)--> smem tile --(row gather)--> registers
 //        --(lie_math.cuh)--> registers --(row scatter)--> smem tile --(16 B coalesced / bulk copy)--> global
@@ -11,9 +12,10 @@
 // L2 policy: an op's input is usually dead after the op, its output is what the next op reads (Exp then
 // Log).  Inputs are therefore read evict-first and outputs stored with normal priority, so the outputs
 // of one launch are still in the 50 MB L2 when the next launch reads them, instead of having been pushed
-// out by the inputs.  The grid is a multiple of the SM count: each CTA gets the same number of elements
-// (chunk), so there is no tail wave.  One element per thread per tile; EPT tiles are batched per barrier
-// to raise bytes in flight.
+// out by the inputs.  The grid is a multiple of the SM count and the CTAs' tile counts differ by at most
+// one, so there is no tail wave.  One element per thread per tile; EPT tiles are batched per barrier
+// to raise bytes in flight.  The plain-load shell (unaligned tensors, tails of <= 3 rows) gives each CTA a
+// contiguous chunk instead.
 #pragma once
 #include "b200pose.h"   // every definition is checked against the generated declaration
 #include <cuda_runtime.h>
@@ -30,7 +32,7 @@ template <typename T, int NIN, int NOUT> struct StreamParams {
   const T* in[NIN];
   T* out[NOUT];
   long long n;       // elements
-  long long chunk;   // elements per CTA (multiple of 4)
+  long long chunk;   // elements per CTA (multiple of 4); plain-load shell only
   int vec_ok;        // all base pointers 16 B aligned
 };
 
@@ -138,10 +140,14 @@ __global__ void __launch_bounds__(THREADS) stream_kernel_tma(StreamParams<typena
   T* s_out = s_in + S * L::IN_WORDS;
   uint64_t* full = reinterpret_cast<uint64_t*>(s_out + OS * L::OUT_WORDS);
 
-  const long long begin = (long long)blockIdx.x * p.chunk;
-  long long end = begin + p.chunk;
-  if (end > p.n) end = p.n;
-  const int ntiles = begin < end ? (int)((end - begin + TILE - 1) / TILE) : 0;
+  // every tile base is a whole number of 16 B units for any row width, as the bulk copies require
+  static_assert((TILE * sizeof(T)) % 16 == 0, "tile bases must stay 16 B aligned");
+  // Tiles are dealt round-robin: CTA b takes tiles b, b + grid, b + 2 grid, ... (grid <= tiles), so only the last tile
+  // of the array can be short, and it is the last tile of the CTA that owns it.
+  // Tile indices fit 32 bits (2^32 tiles would be 1e12 rows).
+  const long long tiles = (p.n + TILE - 1) / TILE;
+  const int ntiles = (int)((tiles - blockIdx.x + gridDim.x - 1) / gridDim.x);
+  auto tile_base = [](int t) { return (long long)(blockIdx.x + (unsigned)t * gridDim.x) * TILE; };   // in rows
   const int tid = threadIdx.x;
 
   // Programmatic dependent launch: our CTAs can be resident while the previous kernel in the stream still runs (see
@@ -158,11 +164,12 @@ __global__ void __launch_bounds__(THREADS) stream_kernel_tma(StreamParams<typena
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   __syncthreads();
 
-  const int last_cnt = ntiles ? (int)(end - begin - (long long)(ntiles - 1) * TILE) : 0;
+  const long long last_left = p.n - tile_base(ntiles - 1);
+  const int last_cnt = (int)(last_left < TILE ? last_left : TILE);
 
   const uint64_t in_policy = l2_policy_evict_first();   // inputs are read once: let them leave L2 first
   auto issue_load = [&](int t, int s) {   // thread 0 only: tile t -> stage s
-    const long long base = begin + (long long)t * TILE;
+    const long long base = tile_base(t);
     const int cnt = (t == ntiles - 1) ? last_cnt : TILE;
     T* dst = s_in + s * L::IN_WORDS;
     const uint32_t b0 = cnt * Op::DI0 * sizeof(T), b1 = Op::NIN > 1 ? cnt * Op::DI1 * sizeof(T) : 0,
@@ -211,7 +218,7 @@ __global__ void __launch_bounds__(THREADS) stream_kernel_tma(StreamParams<typena
     fence_async_smem();
     __syncthreads();
     if (tid == 0) {
-      const long long base = begin + (long long)i * TILE;
+      const long long base = tile_base(i);
       bulk_s2g(p.out[0] + base * Op::DO0, out0, cnt * Op::DO0 * sizeof(T));
       if (Op::NOUT > 1) bulk_s2g(p.out[Op::NOUT > 1 ? 1 : 0] + base * Op::DO1, out1, cnt * Op::DO1 * sizeof(T));
       bulk_commit();
@@ -320,10 +327,7 @@ int launch_stream_tma(const typename Op::T* const* in, typename Op::T* const* ou
   long long tiles = (n + L::TILE - 1) / L::TILE;
   long long slots = (long long)device_info().sms * occ;
   long long grid = tiles < slots ? tiles : slots;
-  long long chunk = (n + grid - 1) / grid;
-  chunk = (chunk + 3) & ~3LL;
-  grid = (n + chunk - 1) / chunk;
-  p.chunk = chunk;
+  p.chunk = 0;   // not read by this shell: CTA b takes tiles b, b + grid, ...
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)grid);
   cfg.blockDim = dim3(THREADS);

@@ -2,12 +2,19 @@
 usage: python tools/ab_stream.py [sym ...]   env: B200POSE_STREAM, B200POSE_CTAS_PER_SM, B200POSE_PDL
        python tools/ab_stream.py --chain     bench.py's step with Log's input warm vs cold in L2
        python tools/ab_stream.py --boundary  cost of one launch boundary (Exp and Log, 8 x N rows in 1 vs 8 launches)
+       python tools/ab_stream.py --ab VAR=VALUE [runs]   --chain and --boundary with and without one switch, alternated
+
+--ab runs `--chain` and `--boundary` in child processes (the shell reads its switches once per process), alternating
+the environment as given (A) with VAR=VALUE added to it (B): A B A B ..., `runs` (default 3) of each, every child waited
+for.  It prints, per side, median and spread over the runs of: one 8e6-row launch of Exp and of Log (steady-state
+streaming, Log's input cold), one launch boundary of each, the chained step with Log's input warm and cold and the L2
+saving; and the card, its power limit and the SM clock sampled under load in each child.
 
 --chain times, on bench.py's ring of 8 batches of 1e6 fp32 elements, Exp(slot j) -> Log(slot j) (the benchmark's
 step: Log reads the SE3 batch Exp has just written) and Exp(slot j) -> Log(slot j+4) (same kernels and bytes, but Log's
 input was written four steps, 416 MB of traffic, earlier and is no longer in L2).  cold - chained is what L2 reuse
 between the two launches saves."""
-import ctypes, os, sys, json
+import ctypes, os, subprocess, sys, json
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from pypose_b200 import _C
@@ -118,10 +125,47 @@ def run_boundary(parts=8, regions=5, trips=200):
     return res
 
 
+def card_under_load(g):
+    """card name, power limit and SM clock, read while replays of graph g keep the GPU busy"""
+    for _ in range(3000): g.replay()
+    q = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--format=csv,noheader",
+                        "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm"], capture_output=True, text=True)
+    torch.cuda.synchronize()
+    return q.stdout.strip() if q.returncode == 0 else "nvidia-smi unavailable"
+
+
+def run_ab(setting, runs=3):
+    var, value = setting.split("=", 1)
+    sides = {"A": dict(os.environ), "B": {**os.environ, var: value}}
+    got = {"A": [], "B": []}
+    for _ in range(runs):
+        for side in "AB":
+            out = subprocess.run([sys.executable, os.path.abspath(__file__), "--ab-child"], env=sides[side],
+                                 capture_output=True, text=True, check=True).stdout
+            got[side].append(json.loads(out.strip().splitlines()[-1]))
+    pick = {"exp_one_launch_us": lambda r: r["exp"]["one_launch_us"], "log_one_launch_us": lambda r: r["log"]["one_launch_us"],
+            "exp_per_boundary_us": lambda r: r["exp"]["per_boundary_us"], "log_per_boundary_us": lambda r: r["log"]["per_boundary_us"],
+            "chained_us": lambda r: r["chained_us"], "cold_us": lambda r: r["cold_us"], "l2_saving_us": lambda r: r["l2_saving_us"]}
+    res = {"B": setting, "card": sorted({r["card"] for side in "AB" for r in got[side]})}
+    for side in "AB":
+        res[side] = {}
+        for k, f in pick.items():
+            v = sorted(f(r) for r in got[side])
+            res[side][k] = {"median": v[len(v) // 2], "min": v[0], "max": v[-1]}
+    return res
+
+
 if __name__ == "__main__":
     args = sys.argv[1:]
     if args == ["--chain"]:
         res = run_chain()
+    elif args == ["--ab-child"]:
+        res = {**run_chain(), **run_boundary()}
+        x, X = torch.randn(N, 6, device=dev), torch.empty(N, 7, device=dev)
+        res["card"] = card_under_load(graph_of(
+            [lambda sp: _C.check(_C.fn("b200_se3_exp_fwd_f32")(x.data_ptr(), X.data_ptr(), N, sp), "exp")]))
+    elif args[:1] == ["--ab"] and len(args) in (2, 3):
+        res = run_ab(args[1], *map(int, args[2:]))
     elif args == ["--boundary"]:
         res = run_boundary()
     else:
