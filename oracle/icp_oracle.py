@@ -102,9 +102,30 @@ class ReduceToBason:
             self.continual = False
 
 
-def icp(source, target, init=None, ord=2, steps=200, patience=5, decreasing=1e-3, tol=1e-5, eps=1e-12):
+def nearest(P, T, ord=2, matcher="brute", block=2048):
+    """Nearest target of every point: P (Np, 3), T (Nt, 3) -> (distances (Np,), indices (Np,)) in fp64.
+
+    "brute": exact, the first minimum (lower index) on ties, in query blocks of `block` rows, so memory stays at
+    block * Nt * 3 values.  "kdtree": scipy's cKDTree, for clouds too large for brute force; the same distances, but an
+    exact tie may pick either index, so use it on clouds whose nearest neighbours are unambiguous."""
+    if matcher == "kdtree":
+        from scipy.spatial import cKDTree
+        d, j = cKDTree(T).query(P, k=1, p=np.inf if ord not in (1, 2) else ord)
+        return d, j
+    d, j = np.empty(len(P)), np.empty(len(P), np.int64)
+    for i in range(0, len(P), block):
+        dd, jj = knn(P[i:i + block], T, 1, ord)
+        d[i:i + block], j[i:i + block] = dd[:, 0], jj[:, 0]
+    return d, j
+
+
+def icp(source, target, init=None, ord=2, steps=200, patience=5, decreasing=1e-3, tol=1e-5, eps=1e-12, matcher="brute",
+        stepper=None):
     """Point-to-point ICP in fp64.  source (..., Ns, 3), target (..., Nt, 3), init (..., 4, 4)/(...,3,4) or None
-    -> A (B, 3, 4) over the flattened broadcast batch, per-step losses (steps, B), batch shape."""
+    -> A (B, 3, 4) over the flattened broadcast batch, per-step losses (steps, B), batch shape.
+
+    Matching runs per batch element (see `nearest` for `matcher`), so memory does not grow with the batch.  `stepper`
+    replaces the ReduceToBason(steps, patience, decreasing, tol) stop rule (any object with `step(loss)` and `continual`)."""
     source, target = np.asarray(source, np.float64), np.asarray(target, np.float64)
     batch = np.broadcast_shapes(source.shape[:-2], target.shape[:-2], () if init is None else np.shape(init)[:-2])
     S = np.broadcast_to(source, batch + source.shape[-2:]).reshape(-1, *source.shape[-2:])
@@ -113,13 +134,16 @@ def icp(source, target, init=None, ord=2, steps=200, patience=5, decreasing=1e-3
     A = np.tile(np.eye(4)[:3], (B, 1, 1))
     if init is not None:
         A = np.broadcast_to(np.asarray(init, np.float64)[..., :3, :], batch + (3, 4)).reshape(B, 3, 4).copy()
-    st = ReduceToBason(steps, patience, decreasing, tol)
+    st = ReduceToBason(steps, patience, decreasing, tol) if stepper is None else stepper
     losses = []
     while st.continual:
         P = S @ A[:, :, :3].transpose(0, 2, 1) + A[:, None, :, 3]
-        d, j = knn(P, Tg, 1, ord)
-        err = d[..., 0].mean(-1)
-        M = np.take_along_axis(Tg, np.repeat(j, 3, -1), -2)
+        err = np.empty(B)
+        M = np.empty_like(P)
+        for b in range(B):
+            d, j = nearest(P[b], Tg[b], ord, matcher)
+            err[b] = d.mean()
+            M[b] = Tg[b][j]
         for b in range(B):
             ms, mt = P[b].mean(0), M[b].mean(0)
             R = kabsch((M[b] - mt).T @ (P[b] - ms), eps)

@@ -45,10 +45,11 @@ template <int ORD, typename T> __device__ __forceinline__ T dist3(T ax, T ay, T 
   if (ORD == 1) return fabs(dx) + fabs(dy) + fabs(dz);
   return fmax(fabs(dx), fmax(fabs(dy), fabs(dz)));
 }
+// ord inf starts from the first coordinate rather than 0: fmax(0, NaN) would be 0, so a NaN point would be at distance 0
 template <int ORD, typename T> __device__ __forceinline__ T distn(const T (&q)[kMaxD], const T* p, int D) {
-  T acc = T(0);
+  T acc = ORD == 0 ? fabs(q[0] - p[0]) : T(0);
 #pragma unroll
-  for (int d = 0; d < kMaxD; ++d)
+  for (int d = ORD == 0 ? 1 : 0; d < kMaxD; ++d)
     if (d < D) {
       const T t = q[d] - p[d];
       acc = ORD == 2 ? fma(t, t, acc) : ORD == 1 ? acc + fabs(t) : fmax(acc, fabs(t));
@@ -88,8 +89,23 @@ __device__ __forceinline__ void stage_tile(Tile<T, DV>& tl, const T* __restrict_
   }
 }
 
+// ord inf: fmax drops a NaN operand, so a point with a NaN coordinate would get a finite distance from the others.  Such a
+// point is made NaN in every coordinate instead, which gives it a NaN distance (as ord 1 and 2 do by arithmetic): it never
+// enters a list.  x: the point's first coordinate, n: its coordinate count.
+template <typename T> __device__ __forceinline__ void nan_spread(T* x, int n) {
+  bool bad = false;
+  for (int d = 0; d < n; ++d) bad = bad || isnan(x[d]);
+  if (bad)
+    for (int d = 0; d < n; ++d) x[d] = pos_inf<T>() - pos_inf<T>();
+}
+template <typename T, int DV, int NT> __device__ __forceinline__ void nan_spread_tile(Tile<T, DV>& tl, int n, int D) {
+  for (int pt = threadIdx.x; pt < n; pt += NT)
+    nan_spread(reinterpret_cast<T*>(tl.p) + pt * (DV == 3 ? 4 : D), DV == 3 ? 3 : D);
+}
+
 // Q queries of this thread against targets [jb, je): the CTA's core loop.  q: query coordinates (D == 3: q[r][0..2]).
-template <typename T, int DV, int K, int ORD, bool LARGEST, int Q, int NT>
+// NANS: make NaN targets NaN in every coordinate for ord inf (k-NN; ICP and the radius mask take finite coordinates only).
+template <typename T, int DV, int K, int ORD, bool LARGEST, int Q, int NT, bool NANS>
 __device__ __forceinline__ void scan_targets(Tile<T, DV>& tl, const T* __restrict__ P, int jb, int je, int D,
                                              const T (&q)[Q][kMaxD], T (&v)[Q][K], int (&id)[Q][K]) {
   for (int j0 = jb; j0 < je; j0 += kTile) {
@@ -97,6 +113,10 @@ __device__ __forceinline__ void scan_targets(Tile<T, DV>& tl, const T* __restric
     __syncthreads();
     stage_tile<T, DV, NT>(tl, P, j0, n, D);
     __syncthreads();
+    if (NANS && ORD == 0) {
+      nan_spread_tile<T, DV, NT>(tl, n, D);
+      __syncthreads();
+    }
 #pragma unroll 4
     for (int jj = 0; jj < n; ++jj) {
       if (DV == 3) {
@@ -112,7 +132,10 @@ __device__ __forceinline__ void scan_targets(Tile<T, DV>& tl, const T* __restric
   }
 }
 
-template <int ORD, typename T> __device__ __forceinline__ T finish_dist(T d) { return ORD == 2 ? sqrt(d) : d; }
+// an empty slot of a `largest` list holds -inf, whose root would be NaN: it stays -inf
+template <int ORD, bool LARGEST, typename T> __device__ __forceinline__ T finish_dist(T d) {
+  return ORD == 2 && (!LARGEST || d >= T(0)) ? sqrt(d) : d;
+}
 
 // grid: nqb query blocks x S splits x B batch elements (flattened in x).  S == 1 writes the results, otherwise the
 // per-split lists (all K entries, ord-2 values still squared) go to pv / pi at ((b S + s) N1 + i) K.
@@ -133,11 +156,19 @@ __global__ void __launch_bounds__(kKnnThreads) knn_kernel(const T* __restrict__ 
     const int i = min((qb * Q + r) * kKnnThreads + (int)threadIdx.x, N1 - 1);
 #pragma unroll
     for (int d = 0; d < kMaxD; ++d) q[r][d] = (DV == 3 ? d < 3 : d < D) ? R[(long long)i * D + d] : T(0);
+    if (ORD == 0) {                                // as nan_spread (unrolled: q stays in registers)
+      bool bad = false;
+#pragma unroll
+      for (int d = 0; d < kMaxD; ++d) bad = bad || ((DV == 3 ? d < 3 : d < D) && isnan(q[r][d]));
+      if (bad)
+#pragma unroll
+        for (int d = 0; d < kMaxD; ++d) q[r][d] = pos_inf<T>() - pos_inf<T>();
+    }
 #pragma unroll
     for (int c = 0; c < K; ++c) { v[r][c] = LARGEST ? -pos_inf<T>() : pos_inf<T>(); id[r][c] = -1; }
   }
   const int jb = s * chunk, je = min(N2, jb + chunk);
-  scan_targets<T, DV, K, ORD, LARGEST, Q, kKnnThreads>(tl, P, jb, je, D, q, v, id);
+  scan_targets<T, DV, K, ORD, LARGEST, Q, kKnnThreads, true>(tl, P, jb, je, D, q, v, id);
 #pragma unroll
   for (int r = 0; r < Q; ++r) {
     const int i = (qb * Q + r) * kKnnThreads + (int)threadIdx.x;
@@ -146,7 +177,7 @@ __global__ void __launch_bounds__(kKnnThreads) knn_kernel(const T* __restrict__ 
       const long long o = ((long long)b * N1 + i) * kout;
 #pragma unroll
       for (int c = 0; c < K; ++c)
-        if (c < kout) { vals[o + c] = finish_dist<ORD>(v[r][c]); idx[o + c] = id[r][c]; }
+        if (c < kout) { vals[o + c] = finish_dist<ORD, LARGEST>(v[r][c]); idx[o + c] = id[r][c]; }
     } else {
       const long long o = (((long long)b * S + s) * N1 + i) * K;
 #pragma unroll
@@ -174,7 +205,7 @@ __global__ void __launch_bounds__(kKnnThreads) knn_merge_kernel(const T* __restr
   }
 #pragma unroll
   for (int c = 0; c < K; ++c)
-    if (c < kout) { vals[g * kout + c] = finish_dist<ORD>(v[c]); idx[g * kout + c] = id[c]; }
+    if (c < kout) { vals[g * kout + c] = finish_dist<ORD, LARGEST>(v[c]); idx[g * kout + c] = id[c]; }
 }
 
 int sm_count() {
@@ -441,7 +472,7 @@ __global__ void __launch_bounds__(NT) icp_match_kernel(const T* __restrict__ src
     v[r][0] = pos_inf<T>();
     id[r][0] = 0;
   }
-  scan_targets<T, 3, 1, ORD, false, Q, NT>(tl, P, 0, Nt, 3, q, v, id);
+  scan_targets<T, 3, 1, ORD, false, Q, NT, false>(tl, P, 0, Nt, 3, q, v, id);
   const double c0x = (double)P[0], c0y = (double)P[1], c0z = (double)P[2];
   double acc[kSums];
 #pragma unroll
@@ -459,7 +490,7 @@ __global__ void __launch_bounds__(NT) icp_match_kernel(const T* __restrict__ src
     for (int a = 0; a < 3; ++a)
 #pragma unroll
       for (int c = 0; c < 3; ++c) acc[6 + 3 * a + c] += t[a] * s[c];
-    acc[15] += (double)finish_dist<ORD>(v[r][0]);
+    acc[15] += (double)finish_dist<ORD, false>(v[r][0]);
     acc[16] += 1.0;
   }
   block_sums<NT>(acc, red);

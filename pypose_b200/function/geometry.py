@@ -125,7 +125,8 @@ def knn(ref, nbr, k=1, ord=2, dim=-1, largest=False, sorted=True):
 
     Coordinates must be finite.  A candidate enters a list only if its distance compares strictly better, so a NaN
     distance never does: a query with NaN coordinates, or with fewer than k targets at a non-NaN distance, gets index -1
-    and value inf (-inf with `largest`) in the slots left empty, where `torch.topk` would rank NaN as the largest value."""
+    and value inf (-inf with `largest`) in the slots left empty, where `torch.topk` would rank NaN as the largest value.
+    A NaN in any coordinate makes the distance NaN, for every `ord`."""
     if not (isinstance(ref, torch.Tensor) and isinstance(nbr, torch.Tensor)):
         raise TypeError("knn: ref and nbr must be tensors")
     if not ref.is_cuda or not nbr.is_cuda:
