@@ -25,6 +25,9 @@ static int solve(const R* Q, const R* p, const R* A, const R* B, const R* c1, co
 
 extern "C" {
 
+// the per-warp shared-memory slab of csrc/lqr.cu, in elements (tests/test_lqr_paths_gpu.py mirrors the launch shape)
+int lqr_host_smem_elems(int ns, int nc) { return lqr_smem_elems(ns, nc); }
+
 int lqr_host_solve(const double* Q, const double* p, const double* A, const double* B, const double* c1, const double* x0,
                    const double* u0, long long nb, int T, int ns, int nc, double* x, double* u, double* cost,
                    double* xtr, int* status) {
