@@ -475,6 +475,29 @@ PCL_OPS = [
       ("long long", "seq", "a number different from the previous call's; appears in host_out[7] when the state is complete")],
      "ICP.forward, pypose/module/icp.py:73-110 (knn -> mean distance -> svdtf -> apply), with "
      "ReduceToBason.step, pypose/utils/stepper.py:58-95, as the stop rule"),
+    ("b200_icp_rec",
+     [("const REAL*", "src", "as b200_icp"), ("long long", "src_bstride", ""), ("const REAL*", "tgt", ""),
+      ("long long", "tgt_bstride", ""), ("const REAL*", "init", ""), ("long long", "init_bstride", ""), ("REAL*", "out", ""),
+      ("REAL*", "err", ""), ("REAL*", "last", ""), ("void*", "ws", ""), ("long long", "B", ""), ("long long", "Ns", ""),
+      ("long long", "Nt", ""), ("int", "ord", ""), ("long long", "first", ""), ("long long", "iters", ""), ("int", "decide", ""),
+      ("long long", "max_steps", ""), ("long long", "patience", ""), ("double", "decreasing", ""), ("double", "tol", ""),
+      ("double*", "host_out", ""), ("long long", "seq", ""),
+      ("void*", "trace", "b200_icp_trace_bytes(B, Ns, iters) bytes: one block per enqueued iteration (A before the step, "
+                         "the Kabsch sums, the match of every source point); skipped iterations leave theirs unwritten")],
+     "ICP.forward as b200_icp, keeping what its backward needs"),
+    ("b200_icp_bwd",
+     [("const REAL*", "src", "(B|1,Ns,3) as given to b200_icp_rec"), ("long long", "src_bstride", "0 = broadcast"),
+      ("const REAL*", "tgt", "(B|1,Nt,3)"), ("long long", "tgt_bstride", "0 = broadcast"),
+      ("const REAL*", "init", "(B|1,7) or NULL"), ("long long", "init_bstride", "7 or 0"),
+      ("const void*", "fwd_ws", "the forward's workspace after its last call (holds A in fp64)"),
+      ("const long long*", "trace_host", "HOST (K): device address of the trace block of iteration 1..K"),
+      ("long long", "K", "iterations run"), ("const REAL*", "grad_out", "(B,7) cotangent of out"),
+      ("REAL*", "grad_src", "(B|1,Ns,3) or NULL"), ("REAL*", "grad_tgt", "(B|1,Nt,3) or NULL"),
+      ("REAL*", "grad_init", "(B|1,7) or NULL"),
+      ("void*", "ws", "b200_icp_bwd_workspace_bytes(B, Ns, Nt, 1 | B) bytes"),
+      ("long long", "B", ""), ("long long", "Ns", ""), ("long long", "Nt", "")],
+     "autograd of ICP.forward, pypose/module/icp.py:73-110 (SE3_Act.backward, mat2SE3, svdtf through torch.linalg.svd), "
+     "matches and iteration count held fixed; deterministic, no float atomics"),
     ("b200_radius_mask",
      [("const REAL*", "pts", "(N,D) points"), ("long long", "N", ""), ("int", "D", "1..16"),
       ("double", "thr", "ord 2: largest squared distance kept (a value of REAL); ord 1 / inf: the radius as a REAL"),

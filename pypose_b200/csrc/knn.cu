@@ -14,9 +14,13 @@
 // fp64 partial sums of the matched pairs; (b) one CTA per batch element reduces its partials in a fixed order, solves the
 // Kabsch step in fp64 (icp_math.cuh) and composes A <- T A; the last CTA evaluates the ReduceToBason rule over the batch
 // and sets the done flag that turns later enqueued iterations into no-ops.
+//
+// ICP backward: the recording variant stores each iteration's matches, A and sums (a trace); the backward walks the
+// iterations in reverse with fp64 cotangents, per-batch fixed-order sums, and a sorted segmented sum for the targets.
 #include <cuda_runtime.h>
 #include <math_constants.h>
 #include <initializer_list>
+#include <cub/device/device_radix_sort.cuh>
 #include "icp_math.cuh"
 
 #define B200_EXPORT extern "C" __attribute__((visibility("default")))
@@ -415,6 +419,12 @@ constexpr int kStWords = 8;
 constexpr int kIcpBig = 256 * 4;           // source points per CTA: 256 threads x 4 queries
 constexpr int kIcpSmall = 128;             // 128 threads x 1 query, when the big CTAs would not fill the GPU
 
+// trace of the recording variant, one block per enqueued iteration: [A before the step (12), sums (17)] x B in fp64, then
+// the match of every source point (B x Ns int32).  An iteration skipped after the done flag leaves its block unwritten.
+constexpr int kRecD = 12 + kSums;
+long long icp_rec_ad_bytes(long long B) { return (B * kRecD * 8 + 255) / 256 * 256; }
+long long icp_rec_block(long long B, long long Ns) { return icp_rec_ad_bytes(B) + (B * Ns * 4 + 255) / 256 * 256; }
+
 bool icp_small(long long B, long long Ns) { return B * ((Ns + kIcpBig - 1) / kIcpBig) < 2LL * sm_count(); }
 long long icp_nx(long long B, long long Ns) {
   const long long per = icp_small(B, Ns) ? kIcpSmall : kIcpBig;
@@ -427,16 +437,16 @@ __device__ __forceinline__ double warp_sum(double x) {
   return x;
 }
 
-// fixed-order block reduction of kSums values; the totals end up in red[0][*] (visible after the final __syncthreads)
-template <int NT> __device__ __forceinline__ void block_sums(double (&acc)[kSums], double (*red)[kSums]) {
+// fixed-order block reduction of NS values; the totals end up in red[0][*] (visible after the final __syncthreads)
+template <int NT, int NS = kSums> __device__ __forceinline__ void block_sums(double (&acc)[NS], double (*red)[NS]) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
 #pragma unroll
-  for (int k = 0; k < kSums; ++k) acc[k] = warp_sum(acc[k]);
+  for (int k = 0; k < NS; ++k) acc[k] = warp_sum(acc[k]);
   if (lane == 0)
 #pragma unroll
-    for (int k = 0; k < kSums; ++k) red[w][k] = acc[k];
+    for (int k = 0; k < NS; ++k) red[w][k] = acc[k];
   __syncthreads();
-  if (threadIdx.x < kSums) {
+  if (threadIdx.x < NS) {
     double s = 0.0;
     for (int i = 0; i < NT / 32; ++i) s += red[i][threadIdx.x];
     red[0][threadIdx.x] = s;          // row 0 is only read again by this thread before the barrier below
@@ -445,10 +455,12 @@ template <int NT> __device__ __forceinline__ void block_sums(double (&acc)[kSums
 }
 
 // (a): k = 1 matching of A source against target and the per-CTA fp64 sums.  grid: nx x B (flattened).
-template <typename T, int ORD, int Q, int NT>
+// REC: also store the match of every source point in rec (B x Ns).
+template <typename T, int ORD, int Q, int NT, bool REC>
 __global__ void __launch_bounds__(NT) icp_match_kernel(const T* __restrict__ src, long long sbs, const T* __restrict__ tgt,
                                                        long long tbs, int Ns, int Nt, const double* __restrict__ A,
-                                                       const double* st, double* __restrict__ part, int nx, int decide) {
+                                                       const double* st, double* __restrict__ part, int nx, int decide,
+                                                       int* __restrict__ rec) {
   if (decide && st[2] == 0.0) return;
   __shared__ Tile<T, 3> tl;
   __shared__ double red[NT / 32][kSums];
@@ -482,6 +494,7 @@ __global__ void __launch_bounds__(NT) icp_match_kernel(const T* __restrict__ src
     const int i = (x * Q + r) * NT + (int)threadIdx.x;
     if (i >= Ns) continue;
     const long long j = id[r][0];
+    if (REC) rec[(long long)b * Ns + i] = (int)j;
     const double s[3] = {(double)q[r][0] - c0x, (double)q[r][1] - c0y, (double)q[r][2] - c0z};
     const double t[3] = {(double)P[j * 3] - c0x, (double)P[j * 3 + 1] - c0y, (double)P[j * 3 + 2] - c0z};
 #pragma unroll
@@ -510,7 +523,7 @@ __global__ void __launch_bounds__(kUpdThreads) icp_update_kernel(const T* __rest
                                                                  const double* __restrict__ part, int nx, double* st,
                                                                  unsigned* ticket, T* last, T* err, T* out, int B,
                                                                  int decide, R2bCtl ctl, double eps, double* host_out,
-                                                                 double seq, int publish) {
+                                                                 double seq, int publish, double* rec) {
   if (decide && st[2] == 0.0) {
     if (publish && host_out && blockIdx.x == 0 && threadIdx.x == 0) icp_publish(st, host_out, seq);
     return;
@@ -530,6 +543,10 @@ __global__ void __launch_bounds__(kUpdThreads) icp_update_kernel(const T* __rest
     const double c0[3] = {(double)P[0], (double)P[1], (double)P[2]};
     double Ab[12], q[4];
     for (int k = 0; k < 12; ++k) Ab[k] = A[b * 12 + k];
+    if (rec) {                                     // trace: A before the step and the sums it is solved from
+      for (int k = 0; k < 12; ++k) rec[b * kRecD + k] = Ab[k];
+      for (int k = 0; k < kSums; ++k) rec[b * kRecD + 12 + k] = red[0][k];
+    }
     icp_step(red[0], c0, eps, Ab);
     for (int k = 0; k < 12; ++k) A[b * 12 + k] = Ab[k];
     err[b] = (T)(red[0][15] / red[0][16]);
@@ -583,14 +600,22 @@ __global__ void icp_init_kernel(const T* __restrict__ init, long long ibs, doubl
   o[3] = (T)q[0]; o[4] = (T)q[1]; o[5] = (T)q[2]; o[6] = (T)q[3];
 }
 
-template <typename T, int ORD>
-void launch_match(const T* src, long long sbs, const T* tgt, long long tbs, long long B, long long Ns, long long Nt,
-                  const double* A, const double* st, double* part, int nx, int decide, cudaStream_t s) {
+template <typename T, int ORD, bool REC>
+void launch_match_r(const T* src, long long sbs, const T* tgt, long long tbs, long long B, long long Ns, long long Nt,
+                    const double* A, const double* st, double* part, int nx, int decide, int* rec, cudaStream_t s) {
   const unsigned grid = (unsigned)(B * nx);
   if (icp_small(B, Ns))
-    icp_match_kernel<T, ORD, 1, kIcpSmall><<<grid, kIcpSmall, 0, s>>>(src, sbs, tgt, tbs, (int)Ns, (int)Nt, A, st, part, nx, decide);
+    icp_match_kernel<T, ORD, 1, kIcpSmall, REC><<<grid, kIcpSmall, 0, s>>>(src, sbs, tgt, tbs, (int)Ns, (int)Nt, A, st, part,
+                                                                          nx, decide, rec);
   else
-    icp_match_kernel<T, ORD, 4, 256><<<grid, 256, 0, s>>>(src, sbs, tgt, tbs, (int)Ns, (int)Nt, A, st, part, nx, decide);
+    icp_match_kernel<T, ORD, 4, 256, REC><<<grid, 256, 0, s>>>(src, sbs, tgt, tbs, (int)Ns, (int)Nt, A, st, part, nx, decide,
+                                                              rec);
+}
+template <typename T, int ORD>
+void launch_match(const T* src, long long sbs, const T* tgt, long long tbs, long long B, long long Ns, long long Nt,
+                  const double* A, const double* st, double* part, int nx, int decide, int* rec, cudaStream_t s) {
+  if (rec) launch_match_r<T, ORD, true>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, rec, s);
+  else launch_match_r<T, ORD, false>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, nullptr, s);
 }
 
 int wait_seq(double* host_out, long long seq, cudaStream_t s) {
@@ -609,9 +634,9 @@ template <typename T>
 int icp_run(const T* src, long long sbs, const T* tgt, long long tbs, const T* init, long long ibs, T* out, T* err, T* last,
             void* ws, long long B, long long Ns, long long Nt, int ord, long long first, long long iters, int decide,
             long long max_steps, long long patience, double decreasing, double tol, double* host_out, long long seq,
-            cudaStream_t s) {
+            void* trace, cudaStream_t s) {
   if (B <= 0) return 0;
-  if (!src || !tgt || !out || !err || !last || !ws || !device_ptrs({src, tgt, init, out, err, last, ws}))
+  if (!src || !tgt || !out || !err || !last || !ws || !device_ptrs({src, tgt, init, out, err, last, ws, trace}))
     return (int)cudaErrorInvalidValue;
   if (Ns <= 0 || Nt <= 0 || Ns > 0x7fffffffLL || Nt > 0x7fffffffLL || (ord != 0 && ord != 1 && ord != 2))
     return (int)cudaErrorInvalidValue;
@@ -625,16 +650,330 @@ int icp_run(const T* src, long long sbs, const T* tgt, long long tbs, const T* i
   if (host_out) reinterpret_cast<volatile double*>(host_out)[kStWords - 1] = -1.0;
   if (first) icp_init_kernel<T><<<(unsigned)((B + 127) / 128), 128, 0, s>>>(init, ibs, A, st, ticket, last, out, (int)B);
   for (long long it = 0; it < iters; ++it) {
-    if (ord == 2) launch_match<T, 2>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, s);
-    else if (ord == 1) launch_match<T, 1>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, s);
-    else launch_match<T, 0>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, s);
+    char* blk = trace ? reinterpret_cast<char*>(trace) + it * icp_rec_block(B, Ns) : nullptr;
+    double* rec_ad = reinterpret_cast<double*>(blk);
+    int* rec_idx = blk ? reinterpret_cast<int*>(blk + icp_rec_ad_bytes(B)) : nullptr;
+    if (ord == 2) launch_match<T, 2>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, rec_idx, s);
+    else if (ord == 1) launch_match<T, 1>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, rec_idx, s);
+    else launch_match<T, 0>(src, sbs, tgt, tbs, B, Ns, Nt, A, st, part, nx, decide, rec_idx, s);
     icp_update_kernel<T><<<(unsigned)B, kUpdThreads, 0, s>>>(tgt, tbs, A, part, nx, st, ticket, last, err, out, (int)B, decide,
-                                                             ctl, eps, host_out, (double)seq, it == iters - 1);
+                                                             ctl, eps, host_out, (double)seq, it == iters - 1, rec_ad);
   }
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
   if (!host_out || iters <= 0) return 0;
   return wait_seq(host_out, seq, s);
+}
+
+
+// ----------------------------------------------------------------------------------------------------------------------
+// ICP backward (DESIGN.md §3.4, "Gradients").  Per batch element b and point i, in fp64: G = the cotangent of the current
+// moved point p_k = A_k s, GS = the source's cotangent through the closing svdtf(source, p_K), C = a point's contribution
+// to its matched target in the current iteration, GT = the target cotangent.  Workspace, each part 256-byte aligned:
+// G, GS, C (B Ns 3) | GT (TB Nt 3) | coef (B x 32) | part (B nx 15) | gi (B x 7) | keys[2], vals[2] (B Ns u32) | CUB.
+// ----------------------------------------------------------------------------------------------------------------------
+constexpr int kBwdThreads = 256, kBwdPer = 4;   // per-CTA sums over 1024 points
+constexpr int kCoef = 32;
+long long icp_bwd_nx(long long Ns) { return (Ns + kBwdThreads * kBwdPer - 1) / (kBwdThreads * kBwdPer); }
+long long al256(long long n) { return (n + 255) / 256 * 256; }
+int key_bits(long long n) {
+  int b = 1;
+  while (b < 32 && (1LL << b) < n) ++b;
+  return b;
+}
+size_t icp_sort_bytes(long long n, int bits) {
+  size_t tb = 0;
+  cub::DoubleBuffer<unsigned> k(nullptr, nullptr), v(nullptr, nullptr);
+  cub::DeviceRadixSort::SortPairs(nullptr, tb, k, v, (int)n, 0, bits);
+  return tb;
+}
+struct IcpBwdWs {
+  double *G, *GS, *C, *GT, *coef, *part, *gi;
+  unsigned *keys[2], *vals[2];
+  void* tmp;
+  size_t tmp_bytes;
+  long long bytes;
+};
+IcpBwdWs icp_bwd_layout(char* base, long long B, long long Ns, long long Nt, long long TB) {
+  IcpBwdWs w;
+  const long long BN = B * Ns;
+  long long o = 0;
+  auto take = [&](long long n) { char* p = base ? base + o : nullptr; o += al256(n); return p; };
+  w.G = (double*)take(BN * 24); w.GS = (double*)take(BN * 24); w.C = (double*)take(BN * 24);
+  w.GT = (double*)take(TB * Nt * 24); w.coef = (double*)take(B * kCoef * 8);
+  w.part = (double*)take(B * icp_bwd_nx(Ns) * 15 * 8); w.gi = (double*)take(B * 7 * 8);
+  for (int k = 0; k < 2; ++k) { w.keys[k] = (unsigned*)take(BN * 4); w.vals[k] = (unsigned*)take(BN * 4); }
+  w.tmp_bytes = icp_sort_bytes(BN, key_bits(TB * Nt));
+  w.tmp = take((long long)w.tmp_bytes);
+  w.bytes = o;
+  return w;
+}
+
+template <typename T> __device__ __forceinline__ void ld3(const T* p, double x[3]) {
+  x[0] = (double)p[0]; x[1] = (double)p[1]; x[2] = (double)p[2];
+}
+__device__ __forceinline__ void aff(const double* A, const double s[3], double p[3]) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) p[c] = fma(A[4 * c], s[0], fma(A[4 * c + 1], s[1], fma(A[4 * c + 2], s[2], A[4 * c + 3])));
+}
+__device__ __forceinline__ void rot(const double* A, const double d[3], double e[3]) {   // rotation part of a 3x4 A
+#pragma unroll
+  for (int c = 0; c < 3; ++c) e[c] = A[4 * c] * d[0] + A[4 * c + 1] * d[1] + A[4 * c + 2] * d[2];
+}
+__device__ __forceinline__ void mv(const double* M, const double x[3], bool tr, double y[3]) {   // y (+)= M x or M^T x
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+    y[r] += tr ? M[r] * x[0] + M[3 + r] * x[1] + M[6 + r] * x[2] : M[3 * r] * x[0] + M[3 * r + 1] * x[1] + M[3 * r + 2] * x[2];
+}
+
+// Per-CTA sums, grid nx x B.  FINAL: over d = s - s_0 and e = R_A d (A = A_K): sum d, sum e, sum e d^T (15).
+// Otherwise: sum g [A s; 1]^T (12, 3x4 row major), g = G.  A: 12 doubles per batch element, `as` apart.
+template <typename T, bool FINAL>
+__global__ void __launch_bounds__(kBwdThreads) icp_bwd_sums_kernel(const T* __restrict__ src, long long sbs, int Ns,
+                                                                   const double* __restrict__ A, int as,
+                                                                   const double* __restrict__ G, double* __restrict__ part,
+                                                                   int nx) {
+  constexpr int NS = FINAL ? 15 : 12;
+  __shared__ double red[kBwdThreads / 32][NS];
+  const int x = blockIdx.x % nx, b = blockIdx.x / nx;
+  const T* S = src + (long long)b * sbs;
+  double a[12], cs[3], acc[NS];
+#pragma unroll
+  for (int k = 0; k < 12; ++k) a[k] = A[(long long)b * as + k];
+  ld3(S, cs);
+#pragma unroll
+  for (int k = 0; k < NS; ++k) acc[k] = 0.0;
+#pragma unroll
+  for (int r = 0; r < kBwdPer; ++r) {
+    const int i = (x * kBwdPer + r) * kBwdThreads + (int)threadIdx.x;
+    if (i >= Ns) continue;
+    double s[3], p[3];
+    ld3(S + (long long)i * 3, s);
+    if (FINAL) {
+      const double d[3] = {s[0] - cs[0], s[1] - cs[1], s[2] - cs[2]};
+      rot(a, d, p);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) { acc[c] += d[c]; acc[3 + c] += p[c]; }
+#pragma unroll
+      for (int r2 = 0; r2 < 3; ++r2)
+#pragma unroll
+        for (int c = 0; c < 3; ++c) acc[6 + 3 * r2 + c] += p[r2] * d[c];
+    } else {
+      aff(a, s, p);
+      const double* g = G + ((long long)b * Ns + i) * 3;
+#pragma unroll
+      for (int r2 = 0; r2 < 3; ++r2) {
+        const double gr = g[r2];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) acc[4 * r2 + c] += gr * p[c];
+        acc[4 * r2 + 3] += gr;
+      }
+    }
+  }
+  block_sums<kBwdThreads, NS>(acc, red);
+  if (threadIdx.x < NS) part[((long long)b * nx + x) * NS + threadIdx.x] = red[0][threadIdx.x];
+}
+
+// One CTA per batch element: the partials in a fixed order, then thread 0 solves the per-batch adjoint.
+// MODE 0: closing svdtf -> coef = [GH 9, md 3, me 3, dms 3, dmt 3]; 1: iteration (rec: its trace) -> coef = [R 9, GH 9,
+// ms 3, mt 3, dms 3, dmt 3]; 2: init -> gi = [sum g, sum p x g, 0].
+template <typename T, int MODE>
+__global__ void __launch_bounds__(kUpdThreads) icp_bwd_batch_kernel(const double* __restrict__ part, int nx,
+                                                                    const T* __restrict__ src, long long sbs,
+                                                                    const T* __restrict__ tgt, long long tbs, int Ns,
+                                                                    const double* __restrict__ rec,
+                                                                    const T* __restrict__ gout, double eps,
+                                                                    double* __restrict__ coef, double* __restrict__ gi) {
+  constexpr int NS = MODE == 0 ? 15 : 12;
+  __shared__ double red[kUpdThreads / 32][NS];
+  const int b = blockIdx.x;
+  double acc[NS];
+#pragma unroll
+  for (int k = 0; k < NS; ++k) acc[k] = 0.0;
+  for (int x = threadIdx.x; x < nx; x += kUpdThreads)
+#pragma unroll
+    for (int k = 0; k < NS; ++k) acc[k] += part[((long long)b * nx + x) * NS + k];
+  block_sums<kUpdThreads, NS>(acc, red);
+  if (threadIdx.x != 0) return;
+  const double* P = red[0];
+  double* c = coef + (long long)b * kCoef;
+  if (MODE == 0) {
+    double cs[3], g[7], GH[3][3];
+    ld3(src + (long long)b * sbs, cs);
+    for (int k = 0; k < 7; ++k) g[k] = (double)gout[(long long)b * 7 + k];
+    icp_final_adj(P, cs, (double)Ns, eps, g, GH, c + 9, c + 12, c + 15, c + 18);
+    for (int k = 0; k < 9; ++k) c[k] = GH[k / 3][k % 3];
+  } else if (MODE == 1) {
+    double c0[3], R[3][3], GH[3][3];
+    ld3(tgt + (long long)b * tbs, c0);
+    icp_iter_adj(rec + (long long)b * kRecD + 12, c0, eps, P, R, GH, c + 18, c + 21, c + 24, c + 27);
+    for (int k = 0; k < 9; ++k) { c[k] = R[k / 3][k % 3]; c[9 + k] = GH[k / 3][k % 3]; }
+  } else {
+    double* o = gi + (long long)b * 7;
+    o[0] = P[3]; o[1] = P[7]; o[2] = P[11];
+    o[3] = P[9] - P[6]; o[4] = P[2] - P[8]; o[5] = P[4] - P[1]; o[6] = 0.0;
+  }
+}
+
+// closing svdtf, one thread per (b, i): G = GH (d - md) + dmt (cotangent of p_K), GS = GH^T (e - me) + dms
+template <typename T>
+__global__ void icp_bwd_final_pts_kernel(const T* __restrict__ src, long long sbs, int Ns, long long BN,
+                                         const double* __restrict__ A, const double* __restrict__ coef,
+                                         double* __restrict__ G, double* __restrict__ GS) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= BN) return;
+  const long long b = g / Ns, i = g - b * Ns;
+  const T* S = src + b * sbs;
+  double cs[3], s[3], e[3];
+  ld3(S, cs);
+  ld3(S + i * 3, s);
+  const double d[3] = {s[0] - cs[0], s[1] - cs[1], s[2] - cs[2]};
+  rot(A + b * 12, d, e);
+  const double* c = coef + b * kCoef;
+  const double x[3] = {d[0] - c[9], d[1] - c[10], d[2] - c[11]}, y[3] = {e[0] - c[12], e[1] - c[13], e[2] - c[14]};
+  double gp[3] = {c[18], c[19], c[20]}, gs[3] = {c[15], c[16], c[17]};
+  mv(c, x, false, gp);
+  mv(c, y, true, gs);
+  for (int k = 0; k < 3; ++k) { G[g * 3 + k] = gp[k]; GS[g * 3 + k] = gs[k]; }
+}
+
+// one iteration, one thread per (b, i): p = A_{k-1} s, y its match; G <- R^T G + GH^T (y - mt) + dms, C = GH (p - ms) + dmt,
+// and the sort pair (target row, b Ns + i) when the target gradient is wanted.
+template <typename T>
+__global__ void icp_bwd_iter_pts_kernel(const T* __restrict__ src, long long sbs, const T* __restrict__ tgt, long long tbs,
+                                        int Ns, int Nt, long long BN, const double* __restrict__ rec,
+                                        const int* __restrict__ idx, const double* __restrict__ coef, double* __restrict__ G,
+                                        double* __restrict__ C, unsigned* __restrict__ keys, unsigned* __restrict__ vals) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= BN) return;
+  const long long b = g / Ns, i = g - b * Ns;
+  const double* c = coef + b * kCoef;
+  const int m = idx[g];
+  double s[3], p[3], y[3];
+  ld3(src + b * sbs + i * 3, s);
+  aff(rec + b * kRecD, s, p);
+  ld3(tgt + b * tbs + (long long)m * 3, y);
+  const double gk[3] = {G[g * 3], G[g * 3 + 1], G[g * 3 + 2]};
+  const double ym[3] = {y[0] - c[21], y[1] - c[22], y[2] - c[23]}, pm[3] = {p[0] - c[18], p[1] - c[19], p[2] - c[20]};
+  double gn[3] = {c[24], c[25], c[26]}, ct[3] = {c[27], c[28], c[29]};
+  mv(c, gk, true, gn);
+  mv(c + 9, ym, true, gn);
+  mv(c + 9, pm, false, ct);
+  for (int k = 0; k < 3; ++k) { G[g * 3 + k] = gn[k]; C[g * 3 + k] = ct[k]; }
+  if (keys) { keys[g] = (unsigned)((tbs ? b : 0) * Nt + m); vals[g] = (unsigned)g; }
+}
+
+// segmented sum over the (target row, point) pairs sorted by row, points in increasing order: the first entry of each
+// row adds the row's contributions to GT in that order.  No atomics: the result does not depend on scheduling.
+__global__ void icp_bwd_scatter_kernel(const unsigned* __restrict__ keys, const unsigned* __restrict__ vals, long long n,
+                                       const double* __restrict__ C, double* __restrict__ GT) {
+  const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const unsigned k = keys[p];
+  if (p > 0 && keys[p - 1] == k) return;
+  double a0 = 0.0, a1 = 0.0, a2 = 0.0;
+  for (long long q = p; q < n && keys[q] == k; ++q) {
+    const double* ct = C + (long long)vals[q] * 3;
+    a0 += ct[0]; a1 += ct[1]; a2 += ct[2];
+  }
+  GT[(long long)k * 3] += a0; GT[(long long)k * 3 + 1] += a1; GT[(long long)k * 3 + 2] += a2;
+}
+
+// source gradient: GS + R_0^T G (G when there is no init), summed over b in order for a broadcast source
+template <typename T>
+__global__ void icp_bwd_src_kernel(const double* __restrict__ G, const double* __restrict__ GS, const double* __restrict__ A0,
+                                   int as, int has_init, long long B, int Ns, int bcast, T* __restrict__ out) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= (bcast ? 1 : B) * Ns) return;
+  const long long b0 = bcast ? 0 : g / Ns, i = g - b0 * Ns, b1 = bcast ? B : b0 + 1;
+  double acc[3] = {0.0, 0.0, 0.0};
+  for (long long b = b0; b < b1; ++b) {
+    const long long e = (b * Ns + i) * 3;
+    const double gk[3] = {G[e], G[e + 1], G[e + 2]};
+    double r[3] = {GS[e], GS[e + 1], GS[e + 2]};
+    if (has_init) {
+      const double* a = A0 + b * as;
+      for (int c = 0; c < 3; ++c) r[c] += a[c] * gk[0] + a[4 + c] * gk[1] + a[8 + c] * gk[2];
+    } else {
+      for (int c = 0; c < 3; ++c) r[c] += gk[c];
+    }
+    for (int c = 0; c < 3; ++c) acc[c] += r[c];
+  }
+  for (int c = 0; c < 3; ++c) out[g * 3 + c] = (T)acc[c];
+}
+
+// rows of w doubles -> T, summed over the B rows in order when `sum` (a broadcast operand)
+template <typename T>
+__global__ void icp_bwd_out_kernel(const double* __restrict__ x, long long rows, int w, int sum, T* __restrict__ out) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= (sum ? w : rows * w)) return;
+  double a = 0.0;
+  if (sum)
+    for (long long r = 0; r < rows; ++r) a += x[r * w + g];
+  else
+    a = x[g];
+  out[g] = (T)a;
+}
+
+unsigned blocks(long long n, int nt) { return (unsigned)((n + nt - 1) / nt); }
+
+template <typename T>
+int icp_bwd_run(const T* src, long long sbs, const T* tgt, long long tbs, const T* init, long long ibs, const void* fwd_ws,
+                const long long* trace_host, long long K, const T* gout, T* gsrc, T* gtgt, T* ginit, void* ws, long long B,
+                long long Ns, long long Nt, cudaStream_t s) {
+  if (B <= 0) return 0;
+  if (!src || !tgt || !fwd_ws || !gout || !ws || (K > 0 && !trace_host) || K < 0 || (ginit && !init) ||
+      !device_ptrs({src, tgt, init, fwd_ws, gout, gsrc, gtgt, ginit, ws}))
+    return (int)cudaErrorInvalidValue;
+  for (long long k = 0; k < K; ++k)
+    if (!trace_host[k] || !device_ptrs({reinterpret_cast<const void*>(trace_host[k])})) return (int)cudaErrorInvalidValue;
+  const long long TB = tbs ? B : 1, BN = B * Ns;
+  if (Ns <= 0 || Nt <= 0 || BN > 0x7fffffffLL || TB * Nt > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+  const IcpBwdWs w = icp_bwd_layout(reinterpret_cast<char*>(ws), B, Ns, Nt, TB);
+  const double* AK = reinterpret_cast<const double*>(fwd_ws) + 2 * kStWords;
+  auto rec = [&](long long k) { return reinterpret_cast<const double*>(trace_host[k]); };   // iteration k + 1
+  const int nx = (int)icp_bwd_nx(Ns);
+  const double eps = sizeof(T) == 4 ? 1e-6 : 1e-12;
+  const unsigned gb = (unsigned)(B * nx), pb = blocks(BN, 256);
+  icp_bwd_sums_kernel<T, true><<<gb, kBwdThreads, 0, s>>>(src, sbs, (int)Ns, AK, 12, nullptr, w.part, nx);
+  icp_bwd_batch_kernel<T, 0><<<(unsigned)B, kUpdThreads, 0, s>>>(w.part, nx, src, sbs, tgt, tbs, (int)Ns, nullptr, gout, eps,
+                                                                  w.coef, nullptr);
+  icp_bwd_final_pts_kernel<T><<<pb, 256, 0, s>>>(src, sbs, (int)Ns, BN, AK, w.coef, w.G, w.GS);
+  if (gtgt) cudaMemsetAsync(w.GT, 0, TB * Nt * 24, s);
+  const int bits = key_bits(TB * Nt);
+  for (long long k = K; k >= 1; --k) {           // iteration k: p_{k-1} -> p_k, trace rec(k - 1); A_k from the next one
+    const double* r = rec(k - 1);
+    const double* Ak = k < K ? rec(k) : AK;
+    const int* idx = reinterpret_cast<const int*>(reinterpret_cast<const char*>(r) + icp_rec_ad_bytes(B));
+    icp_bwd_sums_kernel<T, false><<<gb, kBwdThreads, 0, s>>>(src, sbs, (int)Ns, Ak, k < K ? kRecD : 12, w.G, w.part, nx);
+    icp_bwd_batch_kernel<T, 1><<<(unsigned)B, kUpdThreads, 0, s>>>(w.part, nx, src, sbs, tgt, tbs, (int)Ns, r, nullptr, eps,
+                                                                    w.coef, nullptr);
+    icp_bwd_iter_pts_kernel<T><<<pb, 256, 0, s>>>(src, sbs, tgt, tbs, (int)Ns, (int)Nt, BN, r, idx, w.coef, w.G, w.C,
+                                                  gtgt ? w.keys[0] : nullptr, w.vals[0]);
+    if (gtgt) {
+      cub::DoubleBuffer<unsigned> kb(w.keys[0], w.keys[1]), vb(w.vals[0], w.vals[1]);
+      size_t tb = w.tmp_bytes;
+      const cudaError_t e = cub::DeviceRadixSort::SortPairs(w.tmp, tb, kb, vb, (int)BN, 0, bits, s);
+      if (e != cudaSuccess) return (int)e;
+      icp_bwd_scatter_kernel<<<pb, 256, 0, s>>>(kb.Current(), vb.Current(), BN, w.C, w.GT);
+    }
+  }
+  const double* A0 = K > 0 ? rec(0) : AK;
+  const int a0s = K > 0 ? kRecD : 12;
+  if (ginit) {                                     // p_0 = init (.) source: the Act gradient of init
+    icp_bwd_sums_kernel<T, false><<<gb, kBwdThreads, 0, s>>>(src, sbs, (int)Ns, A0, a0s, w.G, w.part, nx);
+    icp_bwd_batch_kernel<T, 2><<<(unsigned)B, kUpdThreads, 0, s>>>(w.part, nx, src, sbs, tgt, tbs, (int)Ns, nullptr, nullptr,
+                                                                    eps, w.coef, w.gi);
+    const int bc = ibs == 0 && B > 1;
+    icp_bwd_out_kernel<T><<<blocks(bc ? 7 : B * 7, 256), 256, 0, s>>>(w.gi, B, 7, bc, ginit);
+  }
+  if (gsrc) {
+    const int bc = sbs == 0 && B > 1;
+    icp_bwd_src_kernel<T><<<blocks((bc ? 1 : B) * Ns, 256), 256, 0, s>>>(w.G, w.GS, A0, a0s, init != nullptr, B, (int)Ns, bc,
+                                                                         gsrc);
+  }
+  if (gtgt) icp_bwd_out_kernel<T><<<blocks(TB * Nt * 3, 256), 256, 0, s>>>(w.GT, TB * Nt * 3, 1, 0, gtgt);
+  return (int)cudaGetLastError();
 }
 
 }  // namespace
@@ -651,6 +990,16 @@ B200_EXPORT long long b200_knn_workspace_bytes(long long B, long long N1, long l
 B200_EXPORT long long b200_icp_workspace_bytes(long long B, long long Ns) {
   if (B <= 0 || Ns <= 0) return 2 * kStWords * 8;
   return (2 * kStWords + B * 12 + B * icp_nx(B, Ns) * kSums) * 8;
+}
+
+B200_EXPORT long long b200_icp_trace_bytes(long long B, long long Ns, long long iters) {
+  if (B <= 0 || Ns <= 0 || iters <= 0) return 0;
+  return iters * icp_rec_block(B, Ns);
+}
+
+B200_EXPORT long long b200_icp_bwd_workspace_bytes(long long B, long long Ns, long long Nt, long long tgt_batches) {
+  if (B <= 0 || Ns <= 0 || Nt <= 0) return 0;
+  return icp_bwd_layout(nullptr, B, Ns, Nt, tgt_batches > 1 ? B : 1).bytes;
 }
 
 #define B200_KNN_ENTRIES(CT, SFX)                                                                                          \
@@ -670,7 +1019,24 @@ B200_EXPORT long long b200_icp_workspace_bytes(long long B, long long Ns) {
                                  long long max_steps, long long patience, double decreasing, double tol,                   \
                                  double* host_out, long long seq, void* stream) {                                          \
     return icp_run<CT>(src, src_bstride, tgt, tgt_bstride, init, init_bstride, out, err, last, ws, B, Ns, Nt, ord, first,  \
-                       iters, decide, max_steps, patience, decreasing, tol, host_out, seq, (cudaStream_t)stream);          \
+                       iters, decide, max_steps, patience, decreasing, tol, host_out, seq, nullptr, (cudaStream_t)stream); \
+  }                                                                                                                        \
+  B200_EXPORT int b200_icp_rec_##SFX(const CT* src, long long src_bstride, const CT* tgt, long long tgt_bstride,           \
+                                     const CT* init, long long init_bstride, CT* out, CT* err, CT* last, void* ws,         \
+                                     long long B, long long Ns, long long Nt, int ord, long long first, long long iters,   \
+                                     int decide, long long max_steps, long long patience, double decreasing, double tol,   \
+                                     double* host_out, long long seq, void* trace, void* stream) {                         \
+    if (!trace && B > 0 && iters > 0) return (int)cudaErrorInvalidValue;                                                   \
+    return icp_run<CT>(src, src_bstride, tgt, tgt_bstride, init, init_bstride, out, err, last, ws, B, Ns, Nt, ord, first,  \
+                       iters, decide, max_steps, patience, decreasing, tol, host_out, seq, trace, (cudaStream_t)stream);   \
+  }                                                                                                                        \
+  B200_EXPORT int b200_icp_bwd_##SFX(const CT* src, long long src_bstride, const CT* tgt, long long tgt_bstride,           \
+                                     const CT* init, long long init_bstride, const void* fwd_ws,                           \
+                                     const long long* trace_host, long long K, const CT* grad_out, CT* grad_src,           \
+                                     CT* grad_tgt, CT* grad_init, void* ws, long long B, long long Ns, long long Nt,       \
+                                     void* stream) {                                                                       \
+    return icp_bwd_run<CT>(src, src_bstride, tgt, tgt_bstride, init, init_bstride, fwd_ws, trace_host, K, grad_out,        \
+                           grad_src, grad_tgt, grad_init, ws, B, Ns, Nt, (cudaStream_t)stream);                            \
   }
 
 B200_KNN_ENTRIES(float, f32)

@@ -11,6 +11,10 @@ Prints one JSON line per measurement and the card name, power limit and max SM c
   pypose/function/geometry.py:311-313 computes it, on the same GPU where it fits in memory.
 * ICP: a fixed 30 iterations (ReduceToBason(30) with tol < 0 and a patience it cannot reach), device-decided loop; time
   per iteration and end to end (host call to result).
+* ICP gradients (`--grad`, or `--grad-only`): the same runs with the source and target requiring grad and the loss
+  sum W * T.matrix(): the forward with its trace, the backward, forward + backward, and the reference's formulation
+  (oracle/icp_grad_oracle.py: knn through the difference tensor, torch.linalg.svd, autograd) where it fits in memory.
+  The SM clock is sampled right after the timed runs.
 """
 import argparse
 import json
@@ -23,6 +27,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pypose_b200 as pp  # noqa: E402
+from oracle import icp_grad_oracle as O  # noqa: E402
 
 FP_INSTR = {torch.float32: (9, 128), torch.float64: (7, 64)}    # instructions per pair, lanes per SM and clock
 
@@ -98,12 +103,89 @@ def bench_icp(dt, B, N, iters=30):
             "per_iteration_us": t / iters * 1e6, "pairs_per_s": B * N * N * iters / t}
 
 
+def sm_clock():
+    return float(subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm", "--format=csv,noheader,nounits", "-i",
+                                 str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip())
+
+
+def median_time(fn, n=5):
+    runs = []
+    for _ in range(n):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fn()
+        torch.cuda.synchronize()
+        runs.append(time.perf_counter() - t0)
+    return sorted(runs)[len(runs) // 2]
+
+
+def bench_icp_grad(dt, B, N, iters=30):
+    g = torch.Generator(device="cuda").manual_seed(1)
+    xy = torch.rand(B, N, 2, device="cuda", dtype=torch.float64, generator=g) * 10
+    tgt = torch.cat([xy, torch.sin(xy[..., :1]) + torch.cos(0.7 * xy[..., 1:])], -1)
+    tf = pp.se3(0.02 * torch.randn(B, 6, device="cuda", dtype=torch.float64, generator=g)).Exp()
+    src = tf.Inv().unsqueeze(-2).Act(tgt).to(dt).requires_grad_()
+    tgt = tgt.to(dt).requires_grad_()
+    W = torch.randn(B, 4, 4, device="cuda", dtype=dt, generator=None)
+    stepper = pp.utils.ReduceToBason(iters, patience=10 ** 9, tol=-1.0)
+    icp = pp.module.ICP(stepper=stepper)
+    box = {}
+
+    def fwd():
+        box["L"] = (icp(src, tgt).matrix() * W).sum()
+
+    def bwd():
+        torch.autograd.grad(box["L"], [src, tgt])
+
+    def both():
+        fwd()
+        bwd()
+    both()
+    assert stepper.steps == iters
+    t_fwd = median_time(fwd)
+    t_bwd_runs = []
+    for _ in range(5):
+        fwd()
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        bwd()
+        torch.cuda.synchronize()
+        t_bwd_runs.append(time.perf_counter() - t0)
+    t_bwd = sorted(t_bwd_runs)[2]
+    t_both = median_time(both)
+    clk = sm_clock()
+    out = {"what": "icp_grad", "dtype": str(dt).split(".")[1], "B": B, "N": N, "iterations": iters,
+           "forward_with_trace_ms": t_fwd * 1e3, "backward_ms": t_bwd * 1e3, "forward_backward_ms": t_both * 1e3,
+           "sm_clock_mhz_after": clk}
+    box.clear()
+    torch.cuda.empty_cache()
+    try:
+        def reference():
+            T, _ = O.icp(src, tgt, iters, None, 2, "project")
+            torch.autograd.grad((O.Matrix.apply(T) * W).sum(), [src, tgt])
+        reference()
+        out["reference_forward_backward_ms"] = median_time(reference, 3) * 1e3
+    except torch.OutOfMemoryError:
+        out["reference_forward_backward_ms"] = None        # the difference tensor does not fit
+    torch.cuda.empty_cache()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--quick", action="store_true", help="shorter timing windows")
+    ap.add_argument("--grad", action="store_true", help="also the ICP gradient rows")
+    ap.add_argument("--grad-only", action="store_true", help="only the ICP gradient rows")
     a = ap.parse_args()
     info = card()
     print(json.dumps(info), flush=True)
+    if a.grad or a.grad_only:
+        for dt in (torch.float32, torch.float64):
+            for B, N in ((1, 100000), (64, 4096)):
+                print(json.dumps({**bench_icp_grad(dt, B, N), "card": info["card"], "power_limit_w": info["power_limit_w"]}),
+                      flush=True)
+        if a.grad_only:
+            return
     for dt in (torch.float32, torch.float64):
         for B, N1, N2 in ((1, 100000, 100000), (64, 4096, 4096), (1, 20000, 200000)):
             print(json.dumps({**bench_knn(info, dt, B, N1, N2, a.quick), "card": info["card"],
