@@ -14,7 +14,6 @@
 // the step).  A rejected trial (rare) is retried by the host with the state it just read: K1 then starts from the stored
 // blocks instead of re-linearising.  All scalars the decision needs are arguments of that call — the host stays the owner of
 // `param_groups` (users edit the damping between steps), the device computes the update.
-#include <stdlib.h>
 #include "lm_common.cuh"
 #include "comm.cuh"
 #include "tma.cuh"
@@ -939,16 +938,9 @@ static int finish_step(double* host_out, long long seq, cudaStream_t s) {
   }
 }
 
-// B200POSE_REPROJ_STAGED: 0 = register-fed kernels only, 1 (default) = TMA-staged kernel for long row lists,
-// 2 = TMA-staged kernel always (A/B knob for DESIGN.md §3.3)
-static int g_staged_mode = -1;
-static int staged_mode() {
-  if (g_staged_mode < 0) {
-    const char* v = getenv("B200POSE_REPROJ_STAGED");
-    g_staged_mode = v && *v ? atoi(v) : 1;
-  }
-  return g_staged_mode;
-}
+// route of the reprojection step (b200_lm_reproj_staged_mode): 0 = register-fed kernels only, 1 (default) = TMA-staged
+// kernel for long row lists, 2 = TMA-staged kernel always (A/B knob for DESIGN.md §3.3)
+static int g_staged_mode = 1;
 // lanes per camera of the register-fed kernel: 0 = by row count (32 for long lists, else 8); A/B knob (b200_lm_reproj_lanes)
 static int g_reproj_lanes = 0;
 template <typename T, int LPC, typename... A>
@@ -990,7 +982,7 @@ B200_EXPORT int b200_lm_reproj_lanes(int lanes) {
   return prev;
 }
 B200_EXPORT int b200_lm_reproj_staged_mode(int mode) {
-  const int prev = staged_mode();
+  const int prev = g_staged_mode;
   if (mode >= 0) g_staged_mode = mode;
   return prev;
 }
@@ -1007,7 +999,7 @@ B200_EXPORT int b200_lm_reproj_staged_mode(int mode) {
     const HostOut ho = make_host_out(host_out, seq);                                                                  \
     const bool wide = rows >= 384 * ncam;                  /* lanes per camera: 32 for long lists, else 8 */          \
     (void)ws1;                                                                                                        \
-    const int staged = staged_mode();                                                                                 \
+    const int staged = g_staged_mode;                                                                                 \
     if ((staged == 2 || (staged == 1 && wide)) && ((((uintptr_t)pts) | ((uintptr_t)pix)) & 15) == 0) {               \
       int rc = staged_prepare<CT>();                                                                                  \
       if (rc) return rc;                                                                                              \

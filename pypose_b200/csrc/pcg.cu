@@ -10,10 +10,6 @@
 //   update  alpha = rz/pq; x += alpha p; r -= alpha q; z = Minv r; rz' = r.z; rr = r.r; converged / maxiter -> done
 //   dir     beta = rz'/rz; p = z + beta p; q = D p          (D: the block-diagonal part of the operator)
 // Reductions are the deterministic last-block fp64 folds of lm_common.cuh.
-#include <stdlib.h>
-#include <string.h>
-#include <string>
-#include <unordered_map>
 #include "lm_common.cuh"
 #include "comm.cuh"
 
@@ -313,8 +309,7 @@ __global__ void __launch_bounds__(THREADS) cg_vec_small_kernel(const T* __restri
 template <typename T>
 static void launch_cg_vec_small(const T* Minv, const T* D, int dmode, T* x, T* r, T* z, T* p, T* q, T* xbest, double* cg,
                                 int par, long long n, cudaStream_t st) {
-  static const int env = getenv("B200POSE_CG_VEC_THREADS") ? atoi(getenv("B200POSE_CG_VEC_THREADS")) : 0;
-  const int th = env ? env : (n <= 2048 ? 256 : (n <= 3072 ? 512 : 1024));     // measured: 256 beats 1024 at 1e3 rows
+  const int th = n <= 2048 ? 256 : (n <= 3072 ? 512 : 1024);     // measured: 256 beats 1024 at 1e3 rows
   if (th == 256) cg_vec_small_kernel<T, 256><<<1, 256, 0, st>>>(Minv, D, dmode, x, r, z, p, q, xbest, cg, par, n);
   else if (th == 512) cg_vec_small_kernel<T, 512><<<1, 512, 0, st>>>(Minv, D, dmode, x, r, z, p, q, xbest, cg, par, n);
   else cg_vec_small_kernel<T, 1024><<<1, 1024, 0, st>>>(Minv, D, dmode, x, r, z, p, q, xbest, cg, par, n);
@@ -480,60 +475,6 @@ using namespace b200pose;
 
 #define LM_LAUNCH(kern, work, st, ...) kern<<<lm_grid(work, kLmThreads), kLmThreads, 0, (cudaStream_t)(st)>>>(__VA_ARGS__)
 
-// ---- optional CUDA-graph replay of a chunk of iterations (B200POSE_CG_GRAPH=1; off by default) -----------------------
-// A chunk is 45-90 kernels of 4-20 us each with ~4 us between dependent kernels.  Capturing the chunk once per distinct
-// argument tuple (on a private stream: the caller's stream may be the legacy default stream, which cannot be captured)
-// and replaying it with cudaGraphLaunch is not expected to help: the gaps are dependency (drain + launch) latency on the
-// device, not host enqueue cost.
-// Kept as an opt-in because it costs nothing when off.  Any failure of the capture API disables it for the process.
-struct GraphCache {
-  std::unordered_map<std::string, cudaGraphExec_t> map;
-  cudaStream_t cap = nullptr;
-  bool disabled = false;
-};
-static GraphCache& graph_cache() {
-  static thread_local GraphCache c;
-  return c;
-}
-template <typename Key, typename F> static int replay_or_launch(const Key& key, cudaStream_t user, F&& enqueue) {
-  static const bool on = getenv("B200POSE_CG_GRAPH") && atoi(getenv("B200POSE_CG_GRAPH")) != 0;
-  GraphCache& gc = graph_cache();
-  if (!on || gc.disabled) { enqueue(user); return (int)cudaGetLastError(); }
-  const std::string k(reinterpret_cast<const char*>(&key), sizeof(Key));
-  auto it = gc.map.find(k);
-  if (it == gc.map.end()) {
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
-    bool ok = gc.cap || cudaStreamCreateWithFlags(&gc.cap, cudaStreamNonBlocking) == cudaSuccess;
-    ok = ok && cudaStreamBeginCapture(gc.cap, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
-    if (ok) {
-      enqueue(gc.cap);
-      ok = cudaStreamEndCapture(gc.cap, &graph) == cudaSuccess && graph != nullptr;
-    }
-    ok = ok && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess;
-    if (graph) cudaGraphDestroy(graph);
-    if (!ok) {                                   // never seen in practice; keep the solver working regardless
-      gc.disabled = true;
-      cudaGetLastError();
-      enqueue(user);
-      return (int)cudaGetLastError();
-    }
-    if (gc.map.size() >= 64) {                   // bounded: drop everything (addresses changed for good)
-      for (auto& e : gc.map) cudaGraphExecDestroy(e.second);
-      gc.map.clear();
-    }
-    it = gc.map.emplace(k, exec).first;
-  }
-  return (int)cudaGraphLaunch(it->second, user);
-}
-struct PcgKey {                                   // every launch argument of a chunk (padding zeroed by the caller)
-  const void* ptr[20];
-  const void* ptr2;
-  long long num[8];
-  double tol;
-  int tag, dev;
-};
-
 // One chunk of PCG iterations for the pose graph on per-edge blocks (A = M, ia/ib = ei/ej, E edges): the operator walks the
 // edges and scatter-adds.  Single GPU uses pcg2.cu (node-ordered gathers) by default; this is the multi-GPU operator (every
 // rank holds a shard of the edges and the partial products are all-reduced on the device) and the A/B baseline.
@@ -559,111 +500,60 @@ static PcgComm make_pcg_comm(const unsigned long long* bases, int rank, int worl
 }
 constexpr int kPcgChannel = 6;
 
-template <typename CT, bool GATHER>
+template <typename CT>
 static int pgo_pcg_run(const CT* A, const int* ia, const int* ib, long long E, const CT* Minv, const CT* extra, const CT* g,
                        CT* x, CT* r, CT* z, CT* p, CT* q, CT* xbest, double* cg, double* ws, double tol, long long maxiter,
-                       long long first_iter, long long iters, long long n, cudaStream_t user, PcgComm cm) {
+                       long long first_iter, long long iters, long long n, cudaStream_t stream, PcgComm cm) {
   if (n <= 0) return 0;
-  if (cm.on) {
-    const int dmode = cm.P.rank == 0 ? 1 : 0;
-    cudaStream_t stream = user;
-    if (first_iter == 0)
-      LM_LAUNCH(cg_init_kernel<CT>, n, stream, Minv, g, (CT)-1, extra, dmode, x, r, p, q, cg, ws, tol, (double)maxiter, n);
-    for (long long it = first_iter; it < first_iter + iters; ++it) {
-      const int par = (int)(it & 1);
-      if (E > 0) LM_LAUNCH(pcg_pgo_spmv_kernel<CT>, E, stream, A, ia, ib, p, q, cg, E);
+  const int dmode = (!cm.on || cm.P.rank == 0) ? 1 : 0;
+  if (first_iter == 0)
+    LM_LAUNCH(cg_init_kernel<CT>, n, stream, Minv, g, (CT)-1, extra, dmode, x, r, p, q, cg, ws, tol, (double)maxiter, n);
+  for (long long it = first_iter; it < first_iter + iters; ++it) {
+    const int par = (int)(it & 1);
+    if (E > 0) LM_LAUNCH(pcg_pgo_spmv_kernel<CT>, E, stream, A, ia, ib, p, q, cg, E);
+    if (cm.on)
       comm_allreduce_launch<CT>(q, q, n * 6, cm.P, cm.stage, cm.result, kPcgChannel, ++cm.epoch, cm.tickets, cg, stream);
-      if (n <= kVecSmallRows) {
-        launch_cg_vec_small<CT>(Minv, extra, dmode, x, r, z, p, q, xbest, cg, par, n, stream);
-        continue;
-      }
-      LM_LAUNCH(cg_dot_kernel<CT>, n, stream, p, q, cg, ws, n);
-      LM_LAUNCH(cg_update_kernel<CT>, n, stream, Minv, p, q, x, r, z, xbest, cg, ws, par, n);
-      LM_LAUNCH(cg_dir_kernel<CT>, n, stream, z, extra, dmode, p, q, cg, par, n);
+    if (n <= kVecSmallRows) {
+      launch_cg_vec_small<CT>(Minv, extra, dmode, x, r, z, p, q, xbest, cg, par, n, stream);
+      continue;
     }
-    return (int)cudaGetLastError();
+    LM_LAUNCH(cg_dot_kernel<CT>, n, stream, p, q, cg, ws, n);
+    LM_LAUNCH(cg_update_kernel<CT>, n, stream, Minv, p, q, x, r, z, xbest, cg, ws, par, n);
+    LM_LAUNCH(cg_dir_kernel<CT>, n, stream, z, extra, dmode, p, q, cg, par, n);
   }
-  PcgKey key;
-  memset(&key, 0, sizeof(key));
-  const void* ptrs[] = {A, ia, ib, Minv, extra, g, x, r, z, p, q, cg, ws, xbest};
-  for (int i = 0; i < 14; ++i) key.ptr[i] = ptrs[i];
-  key.num[0] = E; key.num[1] = maxiter; key.num[2] = first_iter; key.num[3] = iters; key.num[4] = n;
-  key.tol = tol; key.tag = (GATHER ? 2 : 1) + 16 * (int)sizeof(CT);
-  cudaGetDevice(&key.dev);
-  return replay_or_launch(key, user, [&](cudaStream_t stream) {
-    if (first_iter == 0)
-      LM_LAUNCH(cg_init_kernel<CT>, n, stream, Minv, g, (CT)-1, extra, 1, x, r, p, q, cg, ws, tol, (double)maxiter, n);
-    for (long long it = first_iter; it < first_iter + iters; ++it) {
-      const int par = (int)(it & 1);
-      if (E > 0) LM_LAUNCH(pcg_pgo_spmv_kernel<CT>, E, stream, A, ia, ib, p, q, cg, E);
-      if (n <= kVecSmallRows) {
-        launch_cg_vec_small<CT>(Minv, extra, 1, x, r, z, p, q, xbest, cg, par, n, stream);
-        continue;
-      }
-      LM_LAUNCH(cg_dot_kernel<CT>, n, stream, p, q, cg, ws, n);
-      LM_LAUNCH(cg_update_kernel<CT>, n, stream, Minv, p, q, x, r, z, xbest, cg, ws, par, n);
-      LM_LAUNCH(cg_dir_kernel<CT>, n, stream, z, extra, 1, p, q, cg, par, n);
-    }
-  });
+  return (int)cudaGetLastError();
 }
 template <typename CT>
 static int ba_pcg_run(const CT* Y4, const CT* poses, const int* pidx, const int* cseg, long long split, long long tpi,
                       long long m, const CT* Y4p, const int* cidx_p, const int* pptr, const CT* Hc, const CT* Hpinv,
                       const CT* Minv, const CT* bneg, CT* x, CT* r, CT* z, CT* p, CT* q, CT* t, CT* part, CT* xbest,
                       double* cg, double* ws, double tol, long long maxiter,
-                      long long P, long long first_iter, long long iters, long long n, cudaStream_t user, PcgComm cm) {
+                      long long P, long long first_iter, long long iters, long long n, cudaStream_t stream, PcgComm cm) {
   if (n <= 0) return 0;
-  if (cm.on) {
-    const int dmode = cm.P.rank == 0 ? 2 : 0;
-    cudaStream_t stream = user;
-    if (first_iter == 0)
-      LM_LAUNCH(cg_init_kernel<CT>, n, stream, Minv, bneg, (CT)-1, Hc, dmode, x, r, p, q, cg, ws, tol, (double)maxiter, n);
-    for (long long it = first_iter; it < first_iter + iters; ++it) {
-      const int par = (int)(it & 1);
+  const int dmode = (!cm.on || cm.P.rank == 0) ? 2 : 0;
+  if (first_iter == 0)
+    LM_LAUNCH(cg_init_kernel<CT>, n, stream, Minv, bneg, (CT)-1, Hc, dmode, x, r, p, q, cg, ws, tol, (double)maxiter, n);
+  for (long long it = first_iter; it < first_iter + iters; ++it) {
+    const int par = (int)(it & 1);
+    if (cm.on || m > 0) {         // a rank without observations still takes part in both all-reduces
       // t = Hpp^-1 W^T p: Hpp^-1 is replicated and linear, so the partial sums over this rank's observations are reduced
       LM_LAUNCH(pcg_ba_wtx_gather_kernel<CT>, P * kLanesPerPoint, stream, Y4p, poses, cidx_p, pptr, Hpinv, p,
                 (const CT*)nullptr, (CT)1, t, cg, P);
-      comm_allreduce_launch<CT>(t, t, P * 3, cm.P, cm.stage, cm.result, kPcgChannel, ++cm.epoch, cm.tickets, cg, stream);
+      if (cm.on)
+        comm_allreduce_launch<CT>(t, t, P * 3, cm.P, cm.stage, cm.result, kPcgChannel, ++cm.epoch, cm.tickets, cg, stream);
       ba_wv_seg_launch<CT>(Y4, poses, pidx, cseg, (int)split, (int)tpi, (const CT*)nullptr, t, q, part, cg, n, stream);
-      comm_allreduce_launch<CT>(q, q, n * 6, cm.P, cm.stage, cm.result, kPcgChannel, ++cm.epoch, cm.tickets, cg, stream);
-      if (n <= kVecSmallRows) {
-        launch_cg_vec_small<CT>(Minv, Hc, dmode, x, r, z, p, q, xbest, cg, par, n, stream);
-        continue;
-      }
-      LM_LAUNCH(cg_dot_kernel<CT>, n, stream, p, q, cg, ws, n);
-      LM_LAUNCH(cg_update_kernel<CT>, n, stream, Minv, p, q, x, r, z, xbest, cg, ws, par, n);
-      LM_LAUNCH(cg_dir_kernel<CT>, n, stream, z, Hc, dmode, p, q, cg, par, n);
+      if (cm.on)
+        comm_allreduce_launch<CT>(q, q, n * 6, cm.P, cm.stage, cm.result, kPcgChannel, ++cm.epoch, cm.tickets, cg, stream);
     }
-    return (int)cudaGetLastError();
+    if (n <= kVecSmallRows) {
+      launch_cg_vec_small<CT>(Minv, Hc, dmode, x, r, z, p, q, xbest, cg, par, n, stream);
+      continue;
+    }
+    LM_LAUNCH(cg_dot_kernel<CT>, n, stream, p, q, cg, ws, n);
+    LM_LAUNCH(cg_update_kernel<CT>, n, stream, Minv, p, q, x, r, z, xbest, cg, ws, par, n);
+    LM_LAUNCH(cg_dir_kernel<CT>, n, stream, z, Hc, dmode, p, q, cg, par, n);
   }
-  PcgKey key;
-  memset(&key, 0, sizeof(key));
-  const void* ptrs[] = {Y4, poses, cseg, pidx, Y4p, cidx_p, pptr, Hc, Hpinv, Minv, bneg, x, r, z, p, q, t, cg, ws, part};
-  for (int i = 0; i < 20; ++i) key.ptr[i] = ptrs[i];
-  key.ptr2 = xbest;
-  key.num[0] = m; key.num[1] = maxiter; key.num[2] = first_iter; key.num[3] = iters; key.num[4] = n; key.num[5] = P;
-  key.num[6] = split; key.num[7] = tpi;
-  key.tol = tol; key.tag = 3 + 16 * (int)sizeof(CT);
-  cudaGetDevice(&key.dev);
-  return replay_or_launch(key, user, [&](cudaStream_t stream) {
-    if (first_iter == 0)
-      LM_LAUNCH(cg_init_kernel<CT>, n, stream, Minv, bneg, (CT)-1, Hc, 2, x, r, p, q, cg, ws, tol, (double)maxiter, n);
-    for (long long it = first_iter; it < first_iter + iters; ++it) {
-      const int par = (int)(it & 1);
-      if (m > 0) {
-        LM_LAUNCH(pcg_ba_wtx_gather_kernel<CT>, P * kLanesPerPoint, stream, Y4p, poses, cidx_p, pptr, Hpinv, p,
-                  (const CT*)nullptr, (CT)1, t, cg, P);
-        ba_wv_seg_launch<CT>(Y4, poses, pidx, cseg, (int)split, (int)tpi, (const CT*)nullptr, t, q, part, cg, n, stream);
-      }
-      if (n <= kVecSmallRows) {
-        launch_cg_vec_small<CT>(Minv, Hc, 2, x, r, z, p, q, xbest, cg, par, n, stream);
-        continue;
-      }
-      LM_LAUNCH(cg_dot_kernel<CT>, n, stream, p, q, cg, ws, n);
-      LM_LAUNCH(cg_update_kernel<CT>, n, stream, Minv, p, q, x, r, z, xbest, cg, ws, par, n);
-      LM_LAUNCH(cg_dir_kernel<CT>, n, stream, z, Hc, 2, p, q, cg, par, n);
-    }
-  });
+  return (int)cudaGetLastError();
 }
 
 #define PCG_ABI(SFX, CT)                                                                                              \
@@ -692,9 +582,9 @@ static int ba_pcg_run(const CT* Y4, const CT* poses, const int* pidx, const int*
                                         long long stage, long long result, long long epoch, unsigned* tickets,        \
                                         long long n, void* stream) {                                                  \
     if (!pairs_aligned<CT>(g, x, r, z, p, q, xbest)) return kMisaligned;                                              \
-    return pgo_pcg_run<CT, false>(M, ei, ej, E, Minv, extra, g, x, r, z, p, q, xbest, cg, ws, tol, maxiter,           \
-                                  first_iter, iters, n, (cudaStream_t)stream,                                         \
-                                  make_pcg_comm(bases, rank, world, stage, result, epoch, tickets));                  \
+    return pgo_pcg_run<CT>(M, ei, ej, E, Minv, extra, g, x, r, z, p, q, xbest, cg, ws, tol, maxiter, first_iter,      \
+                           iters, n, (cudaStream_t)stream,                                                            \
+                           make_pcg_comm(bases, rank, world, stage, result, epoch, tickets));                         \
   }                                                                                                                   \
   B200_EXPORT int b200_lm_cg_finish_##SFX(CT* x, const CT* xbest, const double* cg, long long n, void* stream) {      \
     if (n <= 0) return 0;                                                                                             \

@@ -9,7 +9,6 @@
 // elements in registers, thread totals are scanned with order-preserving warp shuffles, warp totals through
 // shared memory.  The group operation is not commutative: every combine keeps (earlier, later) order.
 #include <cuda_runtime.h>
-#include <stdlib.h>
 #include <stdint.h>
 #include "lie_math.cuh"
 #include "b200pose.h"   // every definition is checked against the generated declaration
@@ -872,8 +871,8 @@ static int imu_tma_launch(const T* dt, const T* gyro, const T* acc, const T* ini
 }
 
 // Samples per thread (CH) trades scan overhead (amortised over CH) against coalescing (a thread's CH consecutive
-// samples make every warp access CH-strided).  tools/ab_imu.py compares the choices at 1e3 x 1e4 samples;
-// B200POSE_IMU_CH overrides for A/B runs.
+// samples make every warp access CH-strided).  IMU_ABI fixes it per dtype and route (predict-only / full), from timings
+// of CH = 1, 2 and 4 at 1e3 x 1e4 samples.
 template <typename T, int CH>
 static void imu_launch(const T* dt, const T* gyro, const T* acc, const T* rot, const T* init_rot, long long init_stride,
                        const T* g, T* a, T* Dp, T* Dv, T* Dr, T* Dt, T* w, const T* init_pos, const T* init_vel,
@@ -882,17 +881,10 @@ static void imu_launch(const T* dt, const T* gyro, const T* acc, const T* rot, c
                                                                    a, Dp, Dv, Dr, Dt, w, init_pos, init_vel, pv_stride,
                                                                    rot_out, vel_out, pos_out, F);
 }
-// B200POSE_IMU_TMA / b200_imu_tma_mode: 1 (default) predict-only calls take imu_predict_tma_kernel when they can, 0 never
-static int g_imu_tma = -1;
-static int imu_tma_mode() {
-  if (g_imu_tma < 0) {
-    const char* v = getenv("B200POSE_IMU_TMA");
-    g_imu_tma = v && *v ? atoi(v) : 1;
-  }
-  return g_imu_tma;
-}
+// b200_imu_tma_mode: 1 (default) predict-only calls take imu_predict_tma_kernel when they can, 0 never
+static int g_imu_tma = 1;
 B200_EXPORT int b200_imu_tma_mode(int mode) {
-  const int prev = imu_tma_mode();
+  const int prev = g_imu_tma;
   if (mode >= 0) g_imu_tma = mode;
   return prev;
 }
@@ -903,17 +895,12 @@ B200_EXPORT int b200_imu_tma_mode(int mode) {
                                            const CT* init_vel, long long pv_stride, CT* rot_out, CT* vel_out,          \
                                            CT* pos_out, long long B, long long F, void* s) {                           \
     if (B <= 0 || F <= 0) return 0;                                                                                    \
-    static const int ch_env = getenv("B200POSE_IMU_CH") ? atoi(getenv("B200POSE_IMU_CH")) : 0;                         \
-    const int ch = ch_env ? ch_env : (a ? CH_FULL : CH_PREDICT);                                                       \
-    const int tma_env = imu_tma_mode();                                                                                \
     const uintptr_t bits = (uintptr_t)dt | (uintptr_t)gyro | (uintptr_t)acc | (uintptr_t)rot_out | (uintptr_t)vel_out | \
                            (uintptr_t)pos_out | (uintptr_t)(F * (long long)sizeof(CT));                                \
-    if (tma_env && !a && !rot && rot_out && (bits & 15) == 0) {                                                        \
-      auto tgo = ch == 1 ? imu_tma_launch<CT, 1> : (ch == 4 ? imu_tma_launch<CT, 4> : imu_tma_launch<CT, 2>);          \
-      return tgo(dt, gyro, acc, init_rot, init_stride, gravity3_host, init_pos, init_vel, pv_stride, rot_out, vel_out, \
-                 pos_out, B, F, (cudaStream_t)s);                                                                      \
-    }                                                                                                                  \
-    auto go = ch == 1 ? imu_launch<CT, 1> : (ch == 4 ? imu_launch<CT, 4> : imu_launch<CT, 2>);                         \
+    if (g_imu_tma && !a && !rot && rot_out && (bits & 15) == 0)                                                        \
+      return imu_tma_launch<CT, CH_PREDICT>(dt, gyro, acc, init_rot, init_stride, gravity3_host, init_pos, init_vel,   \
+                                            pv_stride, rot_out, vel_out, pos_out, B, F, (cudaStream_t)s);              \
+    auto go = a ? imu_launch<CT, CH_FULL> : imu_launch<CT, CH_PREDICT>;                                                \
     go(dt, gyro, acc, rot, init_rot, init_stride, gravity3_host, a, Dp, Dv, Dr, Dt, w, init_pos, init_vel, pv_stride,  \
        rot_out, vel_out, pos_out, B, F, (cudaStream_t)s);                                                              \
     return (int)cudaGetLastError();                                                                                    \

@@ -4,8 +4,6 @@ trajectories, plus convergence at the BASELINE.json sizes (configs[2] and config
 Tolerances: fp64 1e-9 relative on sums / 1e-10 on poses; fp32 1e-4 relative on sums, 5e-5 on poses.
 LM converged pose error <= 1e-5 (north_star)."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -785,62 +783,6 @@ def test_pcg_guard_stop_reasons_return_the_best_iterate(dtn, N):
     xs, rr, st, x = _pgo_pcg_by_iteration(-M, ei, ej, Hd, g, 1.0 + 1e-3, 1e-4, 100)
     assert st[CG_DONE] == 2.0 and st[CG_ITERS] == 0.0 and len(xs) == 1
     assert torch.equal(x, torch.zeros_like(x))
-
-
-def _graph_replay_run(out):
-    """Two solves each of a pose graph (scatter route) and of a bundle adjustment, written to `out` (.npz).  Each second
-    solve gets the buffers of the first back from the caching allocator, so under B200POSE_CG_GRAPH=1 it replays the
-    graphs the first one captured."""
-    from pypose_b200.optim import _fused as F
-    dt, scale, dmin, dmax = torch.float64, 1.0 + 1e-4, 1e-6, 1e32
-    rng = np.random.default_rng(25)
-    N = 64
-    gt, init, edges, Z = _pgo_problem(rng, N, 0)
-    edges, Z = edges[::2], Z[::2]             # disjoint pairs: one atomic add per node and product, deterministic sums
-    ei, ej = (torch.from_numpy(edges[:, k].astype(np.int32)).cuda() for k in (0, 1))
-    M, u, _ = ops.lm_pgo_linearize(cu(init, dt), cu(Z, dt), ei, ej, 0, 1.0)
-    Hd, g = ops.lm_pgo_scatter(M, u, ei, ej, N)
-    C, P = 12, 150
-    gt, ptsw, T0, p0, pix, cidx, pidx = _ba_problem(rng, C, P, 3, pix_noise=0.01, consecutive=True)
-    o = np.argsort(cidx, kind="stable")
-    pix, cidx, pidx = pix[o], cidx[o], pidx[o]
-    Td, xd = cu(T0, dt), cu(pix, dt)
-    ci, pi_ = torch.from_numpy(cidx.astype(np.int32)).cuda(), torch.from_numpy(pidx.astype(np.int32)).cuda()
-    geom, _ = _ba_geom(cidx, pidx, xd, C, P, 1, 32)
-    Y4s, rs, Hcc, Hpp, gc, gp, _ = F.ba_linearize_det(Td, cu(p0, dt), xd, pi_, geom, 0, 1.0)
-    res = {}
-    for k in range(2):
-        x, it, pred = F.pgo_solve(M, ei, ej, Hd, g, scale, dmin, dmax, 1e-13, 1000)
-        res.update({f"pgo_x{k}": x.cpu().numpy(), f"pgo_it{k}": it, f"pgo_pred{k}": pred.cpu().numpy(), f"pgo_ptr{k}": x.data_ptr()})
-        del x, pred
-        xc, xp, it, pred = F.ba_solve(Y4s, Td, rs, ci, pi_, geom, Hcc, Hpp, gc, gp, scale, dmin, dmax, 1e-13, 1000)
-        res.update({f"ba_x{k}": np.concatenate([xc.cpu().numpy().ravel(), xp.cpu().numpy().ravel()]), f"ba_it{k}": it,
-                    f"ba_pred{k}": pred.cpu().numpy(), f"ba_ptr{k}": xc.data_ptr()})
-        del xc, xp, pred
-    np.savez(out, **res)
-
-
-def test_cg_graph_replay_is_bit_identical_to_launches(tmp_path):
-    """B200POSE_CG_GRAPH=1 (a chunk of PCG iterations captured once per argument tuple, then replayed) against the default
-    launches, each in its own process (the switch is read once per process): the same x, iteration count and predicted
-    reduction, bit for bit, for the first solve (capture) and for the second on the same buffers (replay)."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    runs = {}
-    for flag in ("0", "1"):
-        out = str(tmp_path / f"graph{flag}.npz")
-        env = dict(os.environ, B200POSE_CG_GRAPH=flag, PYTHONPATH=root)
-        p = subprocess.run([sys.executable, "-c", "import sys; from tests.test_lm_gpu import _graph_replay_run; "
-                            "_graph_replay_run(sys.argv[1])", out], cwd=root, env=env, capture_output=True, text=True,
-                           timeout=600)
-        assert p.returncode == 0, p.stdout + p.stderr
-        runs[flag] = np.load(out)
-    for fam in ("pgo", "ba"):
-        for r in runs.values():
-            assert r[f"{fam}_ptr0"] == r[f"{fam}_ptr1"]                       # the second solve ran on the same buffers
-            assert 0 < r[f"{fam}_it0"] < 1000
-        for k in ("0", "1"):
-            for v in ("x", "it", "pred"):
-                np.testing.assert_array_equal(runs["1"][f"{fam}_{v}{k}"], runs["0"][f"{fam}_{v}{k}"])
 
 
 def _smoke_ba(dev, dtype=torch.float32, tol=1e-6):
