@@ -1,8 +1,8 @@
 """fp64 torch-autograd model of the reference's ICP graph (pypose/module/icp.py:73-110), for the ICP gradient tests.
 
 Test infrastructure only: the package never imports it.  It rebuilds the graph from its definition, on any device:
-* per iteration: k = 1 matching (no gradient), gather, svdtf (centroids, H, torch.linalg.svd, U @ Vh negated as a whole
-  when det = -1, t = mt - R ms), the quaternion of mat2SE3, and SE3 Act;
+* per iteration: k = 1 matching (no gradient; or the matches the caller gives), gather, svdtf (centroids, H,
+  torch.linalg.svd, U @ Vh negated as a whole when det = -1, t = mt - R ms), the quaternion of mat2SE3, and SE3 Act;
 * SE3 Act backward gives the 7-vector of T the gradient [sum g, sum out x g, 0] and the points R^T g;
 * the closing svdtf(source, p_K), whose quaternion takes the sign rule `final`: "reference" (mat2SE3's) or "project"
   (w >= 0, what pp.module.ICP returns);
@@ -104,21 +104,28 @@ def _dist(a, b, ord):
     return d.abs().amax(-1)
 
 
-def icp(source, target, K, init=None, ord=2, final="project"):
-    """The reference's ICP graph with K iterations: returns the 7-vector (batch, 7) and the per-iteration matches."""
+def icp(source, target, K, init=None, ord=2, final="project", matches=None):
+    """The reference's ICP graph with K iterations: returns the 7-vector (batch, 7) and the per-iteration matches.
+    matches: K index tensors (batch, Ns) that iteration k gathers instead of matching (the graph is otherwise the same),
+    so that a run whose nearest neighbours were decided elsewhere (in fp32, say) can be replayed exactly."""
     batch = torch.broadcast_shapes(source.shape[:-2], target.shape[:-2], *([init.shape[:-1]] if init is not None else []))
     temporal = source if init is None else Act.apply(init.unsqueeze(-2), source)
     temporal = temporal.expand(batch + source.shape[-2:])
     tgt = target.expand(batch + target.shape[-2:])
-    matches = []
-    for _ in range(K):
-        with torch.no_grad():
-            idx = _dist(temporal, tgt, ord).argmin(-1)   # ties: the first (lowest) index
-        matches.append(idx)
+    if matches is not None and len(matches) != K:
+        raise ValueError(f"icp: {len(matches)} match tensors for K = {K}")
+    used = []
+    for k in range(K):
+        if matches is not None:
+            idx = matches[k].to(device=tgt.device, dtype=torch.long).reshape(batch + source.shape[-2:-1])
+        else:
+            with torch.no_grad():
+                idx = _dist(temporal, tgt, ord).argmin(-1)   # ties: the first (lowest) index
+        used.append(idx)
         knn = torch.gather(tgt, -2, idx.unsqueeze(-1).expand(idx.shape + (3,)))
         T = svdtf(temporal, knn)
         temporal = Act.apply(T.unsqueeze(-2), temporal)
-    return svdtf(source.expand(batch + source.shape[-2:]), temporal, final), matches
+    return svdtf(source.expand(batch + source.shape[-2:]), temporal, final), used
 
 
 def losses(T, W, probe, w):
@@ -126,10 +133,11 @@ def losses(T, W, probe, w):
     return (Matrix.apply(T) * W).sum(), (Act.apply(T.unsqueeze(-2), probe) * w).sum()
 
 
-def grads(source, target, K, init=None, ord=2, final="project", W=None, probe=None, w=None, which=0):
-    """Gradients of loss `which` (0: matrix, 1: Act) w.r.t. source, target and init (None where not given)."""
+def grads(source, target, K, init=None, ord=2, final="project", W=None, probe=None, w=None, which=0, matches=None):
+    """Gradients of loss `which` (0: matrix, 1: Act) w.r.t. source, target and init (None where not given); matches as
+    in icp()."""
     leaves = [x.detach().clone().requires_grad_() if x is not None else None for x in (source, target, init)]
-    T, _ = icp(leaves[0], leaves[1], K, leaves[2], ord, final)
+    T, _ = icp(leaves[0], leaves[1], K, leaves[2], ord, final, matches)
     L = losses(T, W, probe, w)[which]
     gs = torch.autograd.grad(L, [x for x in leaves if x is not None])
     it = iter(gs)

@@ -90,6 +90,45 @@ def test_oracle_matches_reference_autograd(name, loss):
 
 
 @pytest.mark.parametrize("name", NAMES)
+def test_oracle_given_its_own_matches_is_bit_identical(name):
+    """Replaying the matches the oracle found itself changes nothing: result and every gradient bit for bit."""
+    src, tgt, init, o, K, T = golden_case(name)
+    _, m = O.icp(src, tgt, K, init, o, "reference")
+    assert len(m) == K
+    for loss in (0, 1):
+        a = O.grads(src, tgt, K, init, o, "reference", T("W"), T("probe"), T("w"), loss)
+        b = O.grads(src, tgt, K, init, o, "reference", T("W"), T("probe"), T("w"), loss, matches=m)
+        assert torch.equal(a[0], b[0])
+        for x, y in zip(a[1], b[1]):
+            assert (x is None and y is None) or torch.equal(x, y)
+
+
+@pytest.mark.parametrize("name", NAMES)
+@pytest.mark.parametrize("loss", [0, 1])
+def test_fixed_match_oracle_matches_reference_autograd(name, loss):
+    """The fixed-match oracle, fed the matches of the reference's run, reproduces every golden."""
+    src, tgt, init, o, K, T = golden_case(name)
+    _, m = O.icp(src, tgt, K, init, o, "reference")
+    res, (gs, gt, gi) = O.grads(src, tgt, K, init, o, "reference", T("W"), T("probe"), T("w"), loss, matches=m)
+    np.testing.assert_allclose(res.numpy(), T("result").numpy(), rtol=0, atol=1e-13)
+    for got, key in ((gs, f"gsrc{loss}"), (gt, f"gtgt{loss}")) + (((gi, f"ginit{loss}"),) if init is not None else ()):
+        want = T(key).numpy()
+        np.testing.assert_allclose(got.numpy(), want, rtol=0, atol=1e-12 * np.abs(want).max())
+
+
+def test_fixed_match_oracle_follows_the_given_matches():
+    """Matches other than the nearest ones change the result, and a wrong count of match tensors is refused."""
+    src, tgt, init, o, K, T = golden_case(NAMES[0])
+    res, m = O.icp(src, tgt, K, init, o)
+    shifted = [torch.roll(x, 1, -1) for x in m]
+    other, used = O.icp(src, tgt, K, init, o, matches=shifted)
+    assert all(torch.equal(x, y) for x, y in zip(used, shifted))
+    assert not torch.equal(res, other)
+    with pytest.raises(ValueError):
+        O.icp(src, tgt, K, init, o, matches=m[:-1])
+
+
+@pytest.mark.parametrize("name", NAMES)
 def test_goldens_use_the_agreeing_quaternion_branch(name):
     """In the goldens mat2SE3's quaternion has w >= 0, so the "project" rule of pp.module.ICP gives the same graph."""
     src, tgt, init, o, K, T = golden_case(name)
