@@ -1,6 +1,7 @@
 """numpy oracle of pp.bsr_bsc_matmul (csrc/bsr.cu): the structural output pattern of a BSR × BSC product and its fp64
-values.  Used for the cases the reference is too slow for, and checked against the reference's goldens
-(tests/golden/sparse.npz, oracle/make_golden_sparse.py).
+values, the fp64 gradients of both values arrays, and the triple orders the kernels accumulate in.  Used for the cases
+the reference is too slow for, and checked against the reference's goldens (tests/golden/sparse.npz,
+oracle/make_golden_sparse.py).
 
 A is given as (crow, col, values (nnzA, dm, dn)), B as (ccol, row, values (nnzB, dn, dp)).  Block (i, j) of C exists
 exactly when block row i of A and block column j of B share a stored block index k, stored zero blocks included.
@@ -54,6 +55,36 @@ def product(a_crow, a_col, a_val, b_ccol, b_row, b_val, sm, sp, rows=None):
     out = np.zeros((n, A.shape[1], B.shape[2]))
     np.add.at(out, seg, np.einsum("tij,tjk->tik", A[a], B[b]))
     return crow, col, out
+
+
+def grads(a_crow, a_col, a_val, b_ccol, b_row, b_val, sm, sp, dC):
+    """fp64 dA (nnzA, dm, dn) and dB (nnzB, dn, dp) of <dC, C> for dC (nnz(C), dm, dp) in C's block order:
+    dA[a] += dC[c] B[b]^T and dB[b] += A[a]^T dC[c] over every block product (c, a, b)."""
+    key, a, b = triples(a_crow, a_col, b_ccol, b_row, sp)
+    c = blocks(key)
+    A, B, G = (np.asarray(x, np.float64) for x in (a_val, b_val, dC))
+    dA, dB = np.zeros(A.shape), np.zeros(B.shape)
+    np.add.at(dA, a, np.einsum("tik,tjk->tij", G[c], B[b]))
+    np.add.at(dB, b, np.einsum("tji,tjk->tik", A[a], G[c]))
+    return dA, dB
+
+
+def regroup(key, a, b, by_a, n):
+    """The gradient kernels' triple order (csrc/bsr.cu grad_run): the (i, j, k)-ordered triples of `triples()` sorted
+    stably by a (by_a) or by b, packed as (c << 32) | b or (a << 32) | c.  -> (tri uint64, ptr (n + 1) int64), where
+    entry e of the n entries of A (by_a) or B sums the triples ptr[e] .. ptr[e + 1] - 1."""
+    c = blocks(key)
+    g = np.asarray(a if by_a else b, np.int64)
+    hi, lo = (c, b) if by_a else (a, c)
+    o = np.argsort(g, kind="stable")
+    tri = (np.asarray(hi, np.uint64)[o] << np.uint64(32)) | np.asarray(lo, np.uint64)[o]
+    return tri, np.searchsorted(g[o], np.arange(n + 1)).astype(np.int64)
+
+
+def blocks(key):
+    """output block c of every triple, for keys in (i, j, k) order"""
+    return np.concatenate([[0], np.cumsum(key[1:] != key[:-1])]).astype(np.int64) if len(key) else \
+        np.zeros(0, np.int64)
 
 
 def random_bsr(sm, sn, dm, dn, density, rng, zero_prob=0.0, dtype=np.float64):
