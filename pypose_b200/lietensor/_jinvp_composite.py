@@ -76,10 +76,14 @@ def jlinv_times(grp, x, p):
 
 
 def grad_X(grp, X, p, g):
+    """Left-tangent gradient of g . Jinvp(X, p) with respect to X, evaluated in fp64 for every input dtype: in fp32 the
+    closed-form coefficients lose their digits just above the series switch (c2's numerator theta^2 + 2 cos(theta) - 2
+    is theta^4 / 12, below fp32's rounding of cos(theta) for theta < 0.03), and their autograd derivative, divided by
+    theta^2, turns that into gradient errors of 1e-2 at theta = 0.01."""
     from .ops import _apply
     with torch.enable_grad():
-        Xd = X.detach().requires_grad_(True)
+        Xd = X.detach().double().requires_grad_(True)
         x = _apply(f"{grp}_log_fwd", Xd)
-        out = jlinv_times(grp, x, p.detach())
-        (gX,) = torch.autograd.grad(out, Xd, g)
-    return gX
+        out = jlinv_times(grp, x, p.detach().double())
+        (gX,) = torch.autograd.grad(out, Xd, g.double())
+    return gX.to(X.dtype)
