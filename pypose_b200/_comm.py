@@ -76,9 +76,9 @@ class PeerComm:
 
     @classmethod
     def create(cls, group, device, payload_bytes):
-        """PeerComm or None (no NCCL group / not CUDA / IPC unavailable / disabled with B200POSE_PEER=0)."""
+        """PeerComm or None (no NCCL group / not CUDA / IPC unavailable)."""
         import torch.distributed as dist
-        if group is None or device.type != "cuda" or os.environ.get("B200POSE_PEER", "1") == "0":
+        if group is None or device.type != "cuda":
             return None
         if not (dist.is_available() and dist.is_initialized()):
             return None

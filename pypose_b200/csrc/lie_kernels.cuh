@@ -13,14 +13,13 @@
 // Log).  Inputs are therefore read evict-first and outputs stored with normal priority, so the outputs
 // of one launch are still in the 50 MB L2 when the next launch reads them, instead of having been pushed
 // out by the inputs.  The grid is a multiple of the SM count and the CTAs' tile counts differ by at most
-// one, so there is no tail wave.  One element per thread per tile; EPT tiles are batched per barrier
-// to raise bytes in flight.  The plain-load shell (unaligned tensors, tails of <= 3 rows) gives each CTA a
-// contiguous chunk instead.
+// one, so there is no tail wave.  One element per thread per tile.  The plain-load shell (unaligned tensors,
+// tails of <= 3 rows) gives each CTA a contiguous chunk instead, and batches EPT tiles per barrier to raise
+// bytes in flight.
 #pragma once
 #include "b200pose.h"   // every definition is checked against the generated declaration
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 #include "lie_ops.cuh"
 #include "tma.cuh"
 
@@ -121,19 +120,19 @@ __global__ void __launch_bounds__(kThreads) stream_kernel(StreamParams<typename 
 // Requirements: all base pointers 16 B aligned and every tile a multiple of 4 elements (the launcher
 // guarantees both; the <= 3 element remainder and unaligned tensors go through the v1 kernel).
 // ----------------------------------------------------------------------------
-template <class Op, int S, int OS, int THREADS = kThreads, int EPT = 1> struct TmaLayout {
+template <class Op, int S, int OS> struct TmaLayout {
   using T = typename Op::T;
-  static constexpr int TILE = THREADS * EPT;
+  static constexpr int TILE = kThreads;
   static constexpr int IN_WORDS = TILE * (Op::DI0 + (Op::NIN > 1 ? Op::DI1 : 0) + (Op::NIN > 2 ? Op::DI2 : 0));
   static constexpr int OUT_WORDS = TILE * (Op::DO0 + (Op::NOUT > 1 ? Op::DO1 : 0));
   static constexpr int BYTES = (S * IN_WORDS + OS * OUT_WORDS) * (int)sizeof(T) + 8 * S;
 };
 
-// THREADS threads per CTA, EPT rows per thread per tile (rows tid, tid + THREADS, ...), S input / OS output stages.
-template <class Op, int S, int OS, int THREADS = kThreads, int EPT = 1>
-__global__ void __launch_bounds__(THREADS) stream_kernel_tma(StreamParams<typename Op::T, Op::NIN, Op::NOUT> p) {
+// one row per thread per tile, S input / OS output stages.
+template <class Op, int S, int OS>
+__global__ void __launch_bounds__(kThreads) stream_kernel_tma(StreamParams<typename Op::T, Op::NIN, Op::NOUT> p) {
   using T = typename Op::T;
-  using L = TmaLayout<Op, S, OS, THREADS, EPT>;
+  using L = TmaLayout<Op, S, OS>;
   constexpr int TILE = L::TILE;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   T* s_in = reinterpret_cast<T*>(smem_raw);
@@ -199,9 +198,11 @@ __global__ void __launch_bounds__(THREADS) stream_kernel_tma(StreamParams<typena
     T* out1 = out0 + TILE * Op::DO0;
 
     mbar_wait(&full[s], parity);
+    // One row per thread.  The one-trip loop keeps the compute phase in the plain-load shell's shape: written without
+    // it, nvcc 12.9 fuses different products into FMAs for some ops (SE3 Mul), and the two shells' bits part.
 #pragma unroll
-    for (int e = 0; e < EPT; ++e) {
-      const int row = tid + e * THREADS;
+    for (int e = 0; e < 1; ++e) {
+      const int row = tid + e * kThreads;
       if (row < cnt) {
         T i0[Op::DI0], i1[Op::DI1], i2[Op::DI2], o0[Op::DO0], o1[Op::DO1];
         row_get<Op::DI0>(in0, row, i0);
@@ -282,41 +283,21 @@ int launch_stream_ept(const typename Op::T* const* in, typename Op::T* const* ou
   return (int)cudaGetLastError();
 }
 
-// B200POSE_STREAM=v1 forces the plain-load shell (A/B measurements); B200POSE_CTAS_PER_SM sets the TMA shell's
-// resident CTAs per SM (capped at its occupancy) in place of the default half.
-inline int stream_impl_v1() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("B200POSE_STREAM"); v = (e && e[0] == 'v' && e[1] == '1') ? 1 : 0; }
-  return v;
-}
-inline int stream_pdl() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("B200POSE_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v;
-}
-// 0 = not set: the TMA shell then takes half its occupancy (see launch_stream_tma)
-inline int stream_max_ctas_per_sm() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("B200POSE_CTAS_PER_SM"); v = e ? atoi(e) : 0; if (v < 0) v = 0; }
-  return v;
-}
-
-template <class Op, int S, int OS, int THREADS = kThreads, int EPT = 1>
+template <class Op, int S, int OS>
 int launch_stream_tma(const typename Op::T* const* in, typename Op::T* const* out, long long n, cudaStream_t stream) {
   using T = typename Op::T;
-  using L = TmaLayout<Op, S, OS, THREADS, EPT>;
-  auto kern = stream_kernel_tma<Op, S, OS, THREADS, EPT>;
+  using L = TmaLayout<Op, S, OS>;
+  auto kern = stream_kernel_tma<Op, S, OS>;
   static thread_local int occ_dev[kMaxDevices] = {};
   int& occ = occ_dev[current_device_slot()];
   if (occ == 0) {
     if (L::BYTES > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::BYTES);
     // the largest shared-memory split, so that the SM is not configured for one grid's needs alone
     cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, THREADS, L::BYTES);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, L::BYTES);
     // Half the SM per launch: the CTAs of the next PDL launch in the stream are resident beside this grid while it
     // runs, and start the moment it completes.  The Exp -> Log step measured 1.1 us faster so (DESIGN §3.1, §6).
-    const int cap = stream_max_ctas_per_sm();
-    occ = cap ? (occ < cap ? occ : cap) : occ / 2;
+    occ /= 2;
     if (occ < 1) occ = 1;
   }
   StreamParams<T, Op::NIN, Op::NOUT> p;
@@ -330,14 +311,14 @@ int launch_stream_tma(const typename Op::T* const* in, typename Op::T* const* ou
   p.chunk = 0;   // not read by this shell: CTA b takes tiles b, b + grid, ...
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(THREADS);
+  cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = L::BYTES;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = stream_pdl() ? 1 : 0;
+  cfg.numAttrs = 1;
   cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p);
   return e != cudaSuccess ? (int)e : (int)cudaGetLastError();
 }
@@ -358,7 +339,7 @@ int launch_stream(const typename Op::T* const* in, typename Op::T* const* out, l
   for (int i = 0; i < Op::NIN; ++i) align |= reinterpret_cast<uintptr_t>(in[i]);
   for (int i = 0; i < Op::NOUT; ++i) align |= reinterpret_cast<uintptr_t>(out[i]);
   const long long n4 = n & ~3LL;
-  if ((align & 15) != 0 || n4 == 0 || stream_impl_v1()) return launch_stream_v1<Op>(in, out, n, stream);
+  if ((align & 15) != 0 || n4 == 0) return launch_stream_v1<Op>(in, out, n, stream);
   constexpr int S = sizeof(T) == 4 ? 3 : 2;
   constexpr int OS = 2;
   int rc = launch_stream_tma<Op, S, OS>(in, out, n4, stream);

@@ -6,7 +6,6 @@ linearise, solve, retract, trial loss, `strategy.update`, the accept test and th
 call and the updated ones come back in the 16-double state, which is the step's only device->host read.
 """
 import ctypes
-import os
 
 import torch
 
@@ -109,9 +108,6 @@ GATHER_BYTES = 8 << 20
 def reproj_gather(ncam, world, itemsize):
     """Gather form of the sharded reprojection trial (every rank receives all partial blocks and solves every camera: one
     exchange fewer per trial) while world * ncam blocks stay small; owner form (reduce-scatter + all-gather) beyond."""
-    force = os.environ.get("B200POSE_PEER_GATHER")      # "0" / "1": A/B and tests (must be the same on every rank)
-    if force in ("0", "1"):
-        return force == "1"
     return world * ncam * 28 * itemsize <= GATHER_BYTES
 
 

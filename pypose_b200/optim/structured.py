@@ -15,8 +15,6 @@ Multi-GPU (`group`): PoseInv shards poses (each rank owns its rows; only the sca
 all-reduced).  Reproj shards residuals (each rank accumulates H/g for its rows; H, g and the
 scalars are all-reduced; the 6x6 solves run redundantly on every rank).
 """
-import os
-
 import torch
 
 from .. import _C
@@ -213,9 +211,7 @@ def _device_step(prob, param, strategy):
     if getattr(prob, '_ds_tried', False):
         return None
     prob._ds_tried = True
-    if not param.is_cuda or _lmstep.strategy_kind(strategy) is None:
-        return None
-    if not param.is_contiguous() or os.environ.get("B200POSE_LM_HOST", "0") == "1":
+    if not param.is_cuda or not param.is_contiguous() or _lmstep.strategy_kind(strategy) is None:
         return None
     comm = None
     if prob.group is not None:
@@ -279,11 +275,15 @@ def _unpack21(Hd):
 class PGOProblem(_Problem):
     """Two-pose residuals r_e = Log(Z_e^-1 A^-1 B): block-sparse H, never assembled.
 
-    linearize: per-edge M_e = J^T J and u_e = J^T r (one kernel), diagonal blocks + gradient by atomics.
-    trial:     (H + extra diagonal) D = -g by block-Jacobi preconditioned CG whose matvec walks the edges
-               (csrc/lm.cu lm_pgo_spmv_kernel); the extra diagonal is clamp(diag H) * scale - diag H, i.e. the
-               reference's clamp (optimizer.py:643/657) + cumulative damping (:664/666).
-    Edges may be sharded over a process group: Hd, g, every matvec and the scalars are all-reduced."""
+    Each trial solves (H + extra diagonal) D = -g by block-Jacobi preconditioned CG; the extra diagonal is
+    clamp(diag H) * scale - diag H, i.e. the reference's clamp (optimizer.py:643/657) + cumulative damping (:664/666).
+
+    node-ordered route (unweighted edges on one GPU; csrc/pcg2.cu, lmdrive.cu): every edge owns one slot in each
+               endpoint's adjacency list, the linearisation writes its blocks there and block sums and H products are
+               gathers — no atomics, bit-reproducible.
+    per-edge scatter route (information matrices, or edges sharded over a process group): per-edge M_e = J^T J and
+               u_e = J^T r (one kernel), diagonal blocks + gradient by atomics, a matvec that walks the edges
+               (csrc/lm.cu lm_pgo_spmv_kernel).  With a group, Hd, g, every matvec and the scalars are all-reduced."""
 
     def __init__(self, model, edges, Z, key, group, robust, tol, maxiter, param=None, weight=None):
         self.model, self.key, self.group, self.robust = model, key, group, robust
@@ -295,11 +295,8 @@ class PGOProblem(_Problem):
         self.Z = None if Z is None else Z.tensor().to(self.dtype).reshape(-1, 7).contiguous()
         # information matrices (examples/module/pgo/pgo.py:75 `weight=infos`): (E,6,6) or one (6,6) for all edges
         self.W = None if weight is None else weight.to(self.dtype).reshape(-1, 36).contiguous()
-        # node adjacency (single-GPU device route, csrc/pcg2.cu): every edge owns one slot in each endpoint's list, the
-        # linearisation writes its blocks there and block sums / H products are gathers — no atomics, bit-reproducible.
-        # B200POSE_PGO_SCATTER=1 keeps the round-1 scatter kernels (per-edge blocks + atomics) for A/B measurements.
-        self.node_order = os.environ.get("B200POSE_PGO_SCATTER", "0") != "1"
         self.kind = "pgo"
+        # node adjacency of the node-ordered route: each edge's slot in the lists of its two endpoints
         E = self.ei.shape[0]
         keys = torch.cat([self.ei, self.ej]).long()
         order = torch.sort(keys, stable=True)[1]
@@ -338,7 +335,7 @@ class PGOProblem(_Problem):
 
     def linearize(self):
         nodes = self._nodes()
-        if nodes.is_cuda and self.group is None and self.node_order and self.W is None:
+        if nodes.is_cuda and self.group is None and self.W is None:
             Mn, Hd, g, cur = _fused.pgo_linearize_nodes(self.kind, self, nodes, *self.robust)
             return (Mn,), Hd, g, cur, None
         M, u, cur, unw = self._blocks(nodes)
@@ -416,9 +413,9 @@ class PGOProblem(_Problem):
             return None
         self._pds_tried = True
         nodes = self._nodes()
-        if (not nodes.is_cuda or self.group is not None or not self.node_order or self.W is not None
+        if (not nodes.is_cuda or self.group is not None or self.W is not None
                 or _lmstep.strategy_kind(strategy) is None or not self.param.is_contiguous()
-                or os.environ.get("B200POSE_LM_HOST", "0") == "1" or nodes.get_device() != torch.cuda.current_device()):
+                or nodes.get_device() != torch.cuda.current_device()):
             return None
         self._pds = _lmstep.PgoDeviceStep(self, nodes)
         return self._pds
@@ -623,7 +620,7 @@ class BAProblem(_Problem):
         T, p = self._params()
         if (not T.is_cuda or self.group is not None or _lmstep.strategy_kind(strategy) is None
                 or not self.poses.is_contiguous() or not self.points.is_contiguous() or T.dtype != p.dtype
-                or os.environ.get("B200POSE_LM_HOST", "0") == "1" or T.get_device() != torch.cuda.current_device()):
+                or T.get_device() != torch.cuda.current_device()):
             return None
         self._bds = _lmstep.BaDeviceStep(self, T, p)
         return self._bds

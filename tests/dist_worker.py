@@ -89,9 +89,11 @@ def main():
     present, cams = _lmstep._present_mask(SimpleNamespace(seg=seg, group=True), SimpleNamespace(world=world))
     res["present"], res["cams"] = present.numpy(), cams.numpy()
     res["payload_gather"] = np.array(_lmstep.reproj_payload(1000, 2, 4))
-    os.environ["B200POSE_PEER_GATHER"] = "0"
-    res["payload_owner"] = np.array(_lmstep.reproj_payload(1000, 2, 4))
-    os.environ.pop("B200POSE_PEER_GATHER")
+    gather_bytes, _lmstep.GATHER_BYTES = _lmstep.GATHER_BYTES, 0      # owner form at any size, on every rank
+    try:
+        res["payload_owner"] = np.array(_lmstep.reproj_payload(1000, 2, 4))
+    finally:
+        _lmstep.GATHER_BYTES = gather_bytes
     counts = [torch.zeros(1, dtype=torch.int64) for _ in range(world)]
     dist.all_gather(counts, torch.tensor([ran]))
     res["regions_run"] = torch.cat(counts).numpy()

@@ -65,9 +65,12 @@ def main():
     # blocks + all-gather of the trial poses, gather = every rank receives all blocks and solves every camera
     # ... and both splits: rows as stored (every rank holds rows of every camera) and rows sorted by camera before the
     # split (SURVEY.md §8e: a rank then holds a subset of the cameras; the `present` mask / local camera list route)
+    # the size rule is pinned to one form, the same on every rank: a limit of 0 picks owner, one above every payload gather
+    from pypose_b200.optim import _lmstep
+    gather_bytes = _lmstep.GATHER_BYTES
     for form, split, case, steps in [(f, sp, c, n) for f in ("owner", "gather") for sp in ("stored", "sorted")
                                      for c, n in (("reproj", 4), ("reproj_hard", 6))]:
-        os.environ["B200POSE_PEER_GATHER"] = "1" if form == "gather" else "0"
+        _lmstep.GATHER_BYTES = 1 << 62 if form == "gather" else 0
         tag = case + ("_gather" if form == "gather" else "") + ("_sorted" if split == "sorted" else "")
         pts, pix, cidx = g[f"{case}/pts"], g[f"{case}/pix"], g[f"{case}/cidx"]
         if split == "sorted":
@@ -89,7 +92,7 @@ def main():
         other = [torch.empty_like(mine) for _ in range(world)]
         dist.all_gather(other, mine)
         assert all(torch.equal(o, mine) for o in other), "replicated poses diverged between ranks"
-    os.environ.pop("B200POSE_PEER_GATHER", None)
+    _lmstep.GATHER_BYTES = gather_bytes
     # ---- PGO: edges sharded, nodes replicated
     edges, Z = g["pgo/edges"], g["pgo/Z"]
     E = len(edges)

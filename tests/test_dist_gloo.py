@@ -18,7 +18,7 @@ def _free_port():
     return p
 
 
-def test_sharded_lm_world2_matches_reference(tmp_path, golden_lm):
+def test_sharded_lm_world2_matches_reference_and_sizes_both_exchange_forms(tmp_path, golden_lm):
     out = str(tmp_path / "dist.npz")
     port = str(_free_port())
     procs = []

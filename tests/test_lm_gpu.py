@@ -877,25 +877,25 @@ def test_gauss_newton_structured_route_on_gpu_at_scale():
     assert losses[-1] < 1e-6 * losses[0] + 1e-4, losses
 
 
-@pytest.mark.parametrize("scatter", ["0", "1"])
-def test_lm_pgo_gather_and_scatter_routes(golden_lm, monkeypatch, scatter):
-    """Default: node-ordered gathers (csrc/pcg2.cu, no atomics) — reference trajectory and two bit-identical runs;
-    B200POSE_PGO_SCATTER=1: the per-edge scatter kernels (the multi-GPU operator) — same trajectory."""
-    monkeypatch.setenv("B200POSE_PGO_SCATTER", scatter)
+@pytest.mark.parametrize("route", ["gather", "scatter"])
+def test_lm_pgo_gather_and_scatter_routes(golden_lm, route):
+    """Unweighted: node-ordered gathers (csrc/pcg2.cu, no atomics) — reference trajectory and two bit-identical runs;
+    identity information matrices: the per-edge scatter kernels (the weighted and multi-GPU operator) — same trajectory."""
     g = golden_lm
+    W = torch.eye(6, dtype=torch.float64, device="cuda") if route == "scatter" else None
     finals = []
     for _ in range(2):
         net = pp.module.PoseGraph(pp.SE3(torch.from_numpy(g["pgo/nodes0"].copy()).cuda()))
         inp = (torch.from_numpy(g["pgo/edges"]).cuda(), pp.SE3(torch.from_numpy(g["pgo/Z"].copy()).cuda()))
         opt = pp.optim.LM(net, strategy=pp.optim.strategy.TrustRegion(), solver=pp.optim.solver.PCG(tol=1e-12), sparse=True)
         for k in range(5):
-            loss = opt.step(inp)
-            assert opt._problem is not None and opt._problem.node_order == (scatter == "0")
-            assert (getattr(opt._problem, "_pds", None) is not None) == (scatter == "0")     # native step driver (lmdrive.cu)
+            loss = opt.step(inp, weight=W)
+            assert opt._problem is not None and (opt._problem.W is None) == (route == "gather")
+            assert (getattr(opt._problem, "_pds", None) is not None) == (route == "gather")     # native step driver (lmdrive.cu)
             np.testing.assert_allclose(float(loss), g["pgo/trustregion/loss"][k], rtol=1e-6)
             np.testing.assert_allclose(net.nodes.detach().cpu().numpy(), g["pgo/trustregion/poses"][k], atol=1e-7)
         finals.append(net.nodes.detach().clone())
-    if scatter == "0":
+    if route == "gather":
         assert torch.equal(finals[0], finals[1])
 
 

@@ -599,7 +599,7 @@ def test_device_decision_and_commit_equal_python_strategies(dt, family):
 # ---------------------------------------------------------------------------------------------------------------------
 # end to end: device-decided route against the host-decided route
 @pytest.mark.gpu
-def test_lm_steps_device_route_equal_host_route(monkeypatch):
+def test_lm_steps_device_route_equal_host_route_without_device_step(monkeypatch):
     """2e4 cameras, 5 % gross outliers, Huber, TrustRegion from a poor start, so that the trust region shrinks through
     rejected trials within six LM.steps.  The device-decided route and the host-decided route (lm.cu kernels, decision
     in Python) give the same reject counts, losses to 1e-9 relative and poses to 1e-8 in fp64.  Cameras whose rows are
@@ -607,6 +607,7 @@ def test_lm_steps_device_route_equal_host_route(monkeypatch):
     turn into differences of a few 1e-10 after six steps.  fp32 is not compared end to end: at u kappa > 1 the two fp32
     trajectories part on such cameras from the first step, while every fp32 trial is pinned per camera above."""
     import pypose_b200 as pp
+    from pypose_b200.optim import structured
     dt, ltol, ptol = torch.float64, 1e-9, 1e-8
     rng = np.random.default_rng(41)
     counts = rng.integers(5, 46, 20000)
@@ -616,9 +617,7 @@ def test_lm_steps_device_route_equal_host_route(monkeypatch):
     runs = {}
     for host in (False, True):
         if host:
-            monkeypatch.setenv("B200POSE_LM_HOST", "1")
-        else:
-            monkeypatch.delenv("B200POSE_LM_HOST", raising=False)
+            monkeypatch.setattr(structured.ReprojProblem, "device_step", lambda self, strategy: None)
         net = pp.module.PoseReproj(pp.SE3(cu(init, dt)))
         opt = pp.optim.LM(net, strategy=pp.optim.strategy.TrustRegion(radius=1e6), kernel=pp.optim.kernel.Huber(delta=0.05))
         losses, rejects = [], []

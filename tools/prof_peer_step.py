@@ -37,8 +37,7 @@ with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) a
     torch.cuda.synchronize()
 dist.barrier()
 if rank == 0:
-    print(f"C={C} M={M} world={world}: {dt * 1e6:.1f} us per step (wall clock, converged state), gather form = "
-          f"{os.environ.get('B200POSE_PEER_GATHER', 'auto')}")
+    print(f"C={C} M={M} world={world}: {dt * 1e6:.1f} us per step (wall clock, converged state)")
     rows = [(e.key, e.device_time_total / max(e.count, 1), e.count) for e in prof.key_averages() if e.device_time_total > 0]
     for key, us, cnt in sorted(rows, key=lambda r: -r[1])[:8]:
         print(f"   {us:9.2f} us x{cnt:4d}  {key[:110]}")
