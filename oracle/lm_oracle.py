@@ -10,6 +10,9 @@ Restates pypose/optim/optimizer.py:645-680 (dense LevenbergMarquardt.step) in nu
 tests/test_lm.py checks block == dense, and both against trajectories recorded from the reference's
 own LM (tests/golden/lm.npz, oracle/make_golden_lm.py).
 """
+import math
+from fractions import Fraction
+
 import numpy as np
 
 from . import lie_oracle as O
@@ -188,11 +191,57 @@ def pgo_residual(nodes, Z, ei, ej):
     return O.log("SE3", O.mul("SE3", S, nodes[ej])), S
 
 
-def pgo_jac_blocks(nodes, Z, ei, ej):
+def pgo_jac_blocks(nodes, Z, ei, ej, exact=False):
     """d r / d B = Jl^-1(r) Adj(Z^-1 A^-1) (SE3_Log.backward op.py:389-395 chained with SE3_Mul.backward wrt Y
-    op.py:870-877); d r / d A = -(that) (SE3_Inv.backward op.py:968-973 + SE3_Mul.backward wrt X)."""
+    op.py:870-877); d r / d A = -(that) (SE3_Inv.backward op.py:968-973 + SE3_Mul.backward wrt X).
+    exact=True: Jl^-1 from se3_Jl_inv_exact instead of the reference's closed forms."""
     r, S = pgo_residual(nodes, Z, ei, ej)
-    return r, O.se3_Jl_inv(r) @ O.SE3_Adj(S)
+    return r, (se3_Jl_inv_exact(r) if exact else O.se3_Jl_inv(r)) @ O.SE3_Adj(S)
+
+
+def _series(th2, coef):
+    """sum_n coef[n] th2^n (Horner)."""
+    out = np.zeros_like(th2)
+    for c in coef[::-1]:
+        out = out * th2 + c
+    return out
+
+
+_FACT = [float(math.factorial(k)) for k in range(40)]
+# coefficients in theta^2 of the functions of theta in Jl^-1 (op.py:23-32) and Q (op.py:37-58), to theta^24
+def _bernoulli(n):
+    """B_0 .. B_n as exact fractions (B_1 = -1/2)."""
+    B = [Fraction(1)]
+    for m in range(1, n + 1):
+        B.append(-sum(math.comb(m + 1, k) * B[k] for k in range(m)) / (m + 1))
+    return B
+
+
+_JLINV_SERIES = [float(abs(b) / math.factorial(2 * n)) for n, b in enumerate(_bernoulli(28)[2::2], 1)]   # B_2n / (2n)!
+_Q1_SERIES = [(-1) ** n / _FACT[2 * n + 3] for n in range(13)]        # (th - sin th) / th^3
+_Q2_SERIES = [(-1) ** n / _FACT[2 * n + 4] for n in range(13)]        # (th^2 + 2 cos th - 2) / (2 th^4)
+_Q3_SERIES = [(-1) ** k * (k - 1) / _FACT[2 * k + 1] for k in range(2, 15)]   # (2 th - 3 sin th + th cos th) / (2 th^5)
+
+
+def se3_Jl_inv_exact(x):
+    """se3 Jl^-1 (lie_oracle.se3_Jl_inv) with every coefficient accurate to a few ulps at every angle: the power series
+    below theta = 1, where the closed forms lose up to ~u / theta^4 to cancellation (1e-8 relative at theta = 1e-2 in
+    fp64), the closed forms above it."""
+    tau, phi = x[..., :3], x[..., 3:]
+    th2 = (phi ** 2).sum(-1)[..., None, None]
+    th = np.sqrt(th2)
+    sm = th < 1.0
+    with np.errstate(all="ignore"):
+        c = np.where(sm, _series(th2, _JLINV_SERIES), (1 - th * np.cos(th / 2) / (2 * np.sin(th / 2))) / th2)
+        c1 = np.where(sm, _series(th2, _Q1_SERIES), (th - np.sin(th)) / (th2 * th))
+        c2 = np.where(sm, _series(th2, _Q2_SERIES), (th2 + 2 * np.cos(th) - 2) / (2 * th2 * th2))
+        c3 = np.where(sm, _series(th2, _Q3_SERIES), (2 * th - 3 * np.sin(th) + th * np.cos(th)) / (2 * th2 * th2 * th))
+    P, T = O.vec2skew(phi), O.vec2skew(tau)
+    Ji = np.eye(3) - 0.5 * P + c * (P @ P)
+    Q = (0.5 * T + c1 * (P @ T + T @ P + P @ T @ P) + c2 * (P @ P @ T + T @ P @ P - 3 * P @ T @ P)
+         + c3 * (P @ T @ P @ P + P @ P @ T @ P))
+    Z = np.zeros_like(Ji)
+    return np.concatenate([np.concatenate([Ji, -Ji @ Q @ Ji], -1), np.concatenate([Z, Ji], -1)], -2)
 
 
 def pgo_linearize(nodes, Z, ei, ej, kind=0, delta=1.0, W=None):
@@ -268,14 +317,12 @@ def ba_linearize(poses, points, pix, cidx, pidx, kind=0, delta=1.0):
     sw = np.sqrt(w)
     Jc, Jp, rs = Jc * sw[:, None, None], Jp * sw[:, None, None], r * sw[:, None]
     C, P = poses.shape[0], points.shape[0]
-    Hcc, Hpp, gc, gp = np.zeros((C, 6, 6)), np.zeros((P, 3, 3)), np.zeros((C, 6)), np.zeros((P, 3))
-    np.add.at(Hcc, cidx, np.swapaxes(Jc, -1, -2) @ Jc)
-    np.add.at(Hpp, pidx, np.swapaxes(Jp, -1, -2) @ Jp)
-    np.add.at(gc, cidx, (np.swapaxes(Jc, -1, -2) @ rs[..., None])[..., 0])
-    np.add.at(gp, pidx, (np.swapaxes(Jp, -1, -2) @ rs[..., None])[..., 0])
     iu = np.triu_indices(3)
-    return (Jc.reshape(-1, 12), Jp.reshape(-1, 6), rs, _triu_pack(Hcc), Hpp[:, iu[0], iu[1]], gc, gp,
-            np.array([rho.sum()]))
+    Hcc = _group_sum(cidx, _triu_pack(np.swapaxes(Jc, -1, -2) @ Jc), C)
+    Hpp = _group_sum(pidx, (np.swapaxes(Jp, -1, -2) @ Jp)[:, iu[0], iu[1]], P)
+    gc = _group_sum(cidx, (np.swapaxes(Jc, -1, -2) @ rs[..., None])[..., 0], C)
+    gp = _group_sum(pidx, (np.swapaxes(Jp, -1, -2) @ rs[..., None])[..., 0], P)
+    return Jc.reshape(-1, 12), Jp.reshape(-1, 6), rs, Hcc, Hpp, gc, gp, np.array([rho.sum()])
 
 
 def ba_wtx(Jc, Jp, cidx, pidx, x, npts):
@@ -419,3 +466,220 @@ def reproj2_dense_jac(nodes, pts, ia, ib, intr=README_INTR):
         D[2 * k:2 * k + 2, 7 * ia[k]:7 * ia[k] + 6] += J[k]
         D[2 * k:2 * k + 2, 7 * ib[k]:7 * ib[k] + 6] -= J[k]
     return D
+
+
+# ------------------------------------------------------------------ error scales of the linearisations (sum of |term|)
+# A kernel that computes an entry as a sum of products in a dtype with unit roundoff u is off by at most about
+# u * (the sum of the absolute values of those products).  The *_terms companions return that sum per output entry.  Each
+# factor enters with its own such scale, obtained by evaluating the factor's formula on absolute values: a translation
+# R^T (t_b - t_a) is counted as |R^T| (|t_b| + |t_a|), a projection's numerator fx y.x + sk y.y as |fx| |y.x| + |sk| |y.y|,
+# and a robust weight with its relative sensitivity 2 |r|_abs / delta to the rounding of |r|^2 (kinds 1-5).
+def _rot(q):
+    return O.SO3_Adj(q)
+
+
+def _abs_skew(v):
+    return np.abs(O.vec2skew(v))
+
+
+def _group_sum(idx, vals, n):
+    """Row sums of vals per value of idx (np.bincount per column: fast at 1e6 rows)."""
+    vals = vals.reshape(len(idx), int(np.prod(vals.shape[1:])))
+    return np.stack([np.bincount(idx, weights=vals[:, q], minlength=n) for q in range(vals.shape[1])], 1)
+
+
+def _weight_factor(kind, delta, rabs):
+    if kind in (1, 2, 3, 4, 5):
+        return 1.0 + 2.0 * np.sqrt((rabs ** 2).sum(-1)) / delta
+    return np.ones(rabs.shape[0])
+
+
+def _rho_terms(kind, delta, x):
+    """Sum of |term| of rho(x) itself: PseudoHuber 2 d^2 (q - 1) and SoftLOne 2 (d q - 1) cancel to O(x) from O(1) terms."""
+    if kind == 2:
+        return 2 * delta * delta * (np.sqrt(x / delta ** 2 + 1) + 1)
+    if kind == 4:
+        return 2 * (delta * np.sqrt(1 / delta ** 2 + x) + 1)
+    return np.abs(robust(kind, delta, x)[0])
+
+
+def rows_linearize(J, r, grp, n, kind=0, delta=1.0, W=None):
+    """M (n, 21) = sum w J^T W J, u (n, 6) = sum w J^T W r and the cost sum rho(|r|^2) over the residual rows (J (m, d, 6),
+    r (m, d), information matrices W (m, d, d) or None) grouped by grp into n blocks: the assembly of pgo_linearize /
+    reproj2_accum for Jacobians computed once."""
+    rho, w = robust(kind, delta, (r ** 2).sum(-1))
+    WJ = J if W is None else W @ J
+    Wr = r if W is None else (W @ r[..., None])[..., 0]
+    iu = np.triu_indices(6)
+    M = np.einsum('mka,mkb->mab', J, WJ)[:, iu[0], iu[1]] * w[:, None]
+    u = np.einsum('mka,mk->ma', J, Wr) * w[:, None]
+    return _group_sum(grp, M, n), _group_sum(grp, u, n), np.array([rho.sum()])
+
+
+def rows_terms(J, r, Jabs, rabs, grp, n, kind=0, delta=1.0, W=None):
+    """Sum of |term| of M (n, 21) = sum w J^T J, u (n, 6) = sum w J^T r and the cost sum rho(|r|^2) over the residual rows
+    (J (m, d, 6), r (m, d)) grouped by grp into n blocks, from the magnitudes Jabs / rabs of the factors."""
+    rho, w = robust(kind, delta, (r ** 2).sum(-1))
+    ww = w * _weight_factor(kind, delta, rabs)
+    iu = np.triu_indices(6)
+    WJ = Jabs if W is None else np.abs(W) @ Jabs
+    Wr = rabs if W is None else (np.abs(W) @ rabs[..., None])[..., 0]
+    MM = np.einsum('mka,mkb->mab', Jabs, WJ)[:, iu[0], iu[1]] * ww[:, None]
+    uu = np.einsum('mka,mk->ma', Jabs, Wr) * ww[:, None]
+    cost = _rho_terms(kind, delta, (r ** 2).sum(-1)).sum() + (w * 2 * (np.abs(r) * rabs).sum(-1)).sum()
+    return _group_sum(grp, MM, n), _group_sum(grp, uu, n), np.array([cost])
+
+
+def pgo_terms(nodes, Z, ei, ej):
+    """Magnitudes (Jabs (E,6,6), rabs (E,6)) of the factors of pgo_jac_blocks."""
+    r, S = pgo_residual(nodes, Z, ei, ej)
+    A, B = nodes[ei], nodes[ej]
+    RZt, RAt = np.swapaxes(_rot(Z[:, 3:]), -1, -2), np.swapaxes(_rot(A[:, 3:]), -1, -2)
+    tabs = (np.abs(RZt) @ ((np.abs(RAt) @ (np.abs(B[:, :3]) + np.abs(A[:, :3]))[..., None])[..., 0] + np.abs(Z[:, :3]))[..., None])[..., 0]
+    rabs = np.concatenate([(np.abs(O.so3_Jl_inv(r[:, 3:])) @ tabs[..., None])[..., 0], np.abs(r[:, 3:]) + 1.0], -1)
+    # R_S = R_Z^T R_A^T R_B and the rotation of r come from products of unit quaternions: their entries carry O(1) terms
+    # even where the residual rotation is small
+    Jl = np.abs(O.se3_Jl_inv(r))
+    Jl[:, :3, 3:] += _abs_skew(rabs[:, :3])
+    for k in (slice(0, 3), slice(3, 6)):
+        Jl[:, k, k] += 0.5 * _abs_skew(rabs[:, 3:])
+    RS = np.abs(np.swapaxes(_rot(Z[:, 3:]), -1, -2)) @ np.abs(RAt) @ np.abs(_rot(B[:, 3:]))
+    AdjA = np.concatenate([np.concatenate([RS, _abs_skew(tabs) @ RS], -1),
+                           np.concatenate([np.zeros_like(RS), RS], -1)], -2)
+    return Jl @ AdjA, rabs
+
+
+def pgo_linearize_terms(nodes, Z, ei, ej, kind=0, delta=1.0, W=None):
+    """Sum of |term| of each output of pgo_linearize (per edge; with W the weighted pair first, as pgo_linearize)."""
+    r, J = pgo_jac_blocks(nodes, Z, ei, ej)
+    Jabs, rabs = pgo_terms(nodes, Z, ei, ej)
+    E = len(ei)
+    M, u, cost = rows_terms(J, r, Jabs, rabs, np.arange(E), E, kind, delta)
+    if W is None:
+        return M, u, cost
+    Mw, uw, _ = rows_terms(J, r, Jabs, rabs, np.arange(E), E, kind, delta, np.broadcast_to(W.reshape(-1, 6, 6), J.shape))
+    return Mw, uw, M, u, cost
+
+
+def _proj_abs(y, yabs, intr):
+    """Magnitudes of d proj / d y (m,2,3) and of proj(y) (m,2) for intrinsics (fx, sk, cx, fy, cy)."""
+    fx, sk, cx, fy, cy = (abs(v) for v in intr)
+    z = np.abs(y[:, 2])
+    zf = yabs[:, 2] / z                                     # the rounding of 1 / y.z, relative
+    m = len(y)
+    d = np.zeros((m, 2, 3))
+    d[:, 0, 0], d[:, 0, 1] = fx / z, sk / z
+    d[:, 0, 2] = (fx * yabs[:, 0] + sk * yabs[:, 1]) / z ** 2
+    d[:, 1, 1], d[:, 1, 2] = fy / z, fy * yabs[:, 1] / z ** 2
+    p = np.stack([(fx * yabs[:, 0] + sk * yabs[:, 1]) / z + cx, fy * yabs[:, 1] / z + cy], -1)
+    return d * zf[:, None, None], p * zf[:, None]
+
+
+def reproj2_terms(nodes, pts, pix, ia, ib, intr=README_INTR):
+    """Magnitudes (Jabs (m,2,6), rabs (m,2)) of the factors of reproj2_jac_rows / reproj2_residual."""
+    _, y = reproj2_residual(nodes, pts, pix, ia, ib, intr)
+    Ta, Tb = nodes[ia], nodes[ib]
+    Ra, Rbt = np.abs(_rot(Ta[:, 3:])), np.abs(np.swapaxes(_rot(Tb[:, 3:]), -1, -2))
+    wabs = (Ra @ np.abs(pts)[..., None])[..., 0] + np.abs(Ta[:, :3])
+    yabs = (Rbt @ (wabs + np.abs(Tb[:, :3]))[..., None])[..., 0]
+    dpi, pabs = _proj_abs(y, yabs, intr)
+    tinv = (Rbt @ np.abs(Tb[:, :3])[..., None])[..., 0]
+    Adj = np.concatenate([np.concatenate([Rbt, _abs_skew(tinv) @ Rbt], -1),
+                          np.concatenate([np.zeros_like(Rbt), Rbt], -1)], -2)
+    dy = np.concatenate([np.broadcast_to(np.eye(3), (len(y), 3, 3)), _abs_skew(yabs)], -1)
+    return dpi @ dy @ Adj, pabs + np.abs(pix)
+
+
+def reproj2_accum_terms(nodes, pts, pix, pseg, pa, pb, intr=README_INTR, kind=0, delta=1.0):
+    """Sum of |term| of each output of reproj2_accum (per pair)."""
+    E = len(pa)
+    pe = np.repeat(np.arange(E), np.diff(pseg))
+    ia, ib = np.asarray(pa)[pe], np.asarray(pb)[pe]
+    r, _ = reproj2_residual(nodes, pts, pix, ia, ib, intr)
+    J = reproj2_jac_rows(nodes, pts, ia, ib, intr)
+    Jabs, rabs = reproj2_terms(nodes, pts, pix, ia, ib, intr)
+    return rows_terms(J, r, Jabs, rabs, pe, E, kind, delta)
+
+
+def ba_terms(poses, points, pix, cidx, pidx):
+    """Magnitudes (Jc_abs (m,2,6), Jp_abs (m,2,3), rabs (m,2)) of the factors of ba_jac_rows / ba_residual."""
+    y = O.act("SE3", poses[cidx], points[pidx])
+    R = np.abs(_rot(poses[cidx][:, 3:]))
+    yabs = (R @ np.abs(points[pidx])[..., None])[..., 0] + np.abs(poses[cidx][:, :3])
+    dpi, pabs = _proj_abs(y, yabs, README_INTR)
+    dy = np.concatenate([np.broadcast_to(np.eye(3), (len(y), 3, 3)), _abs_skew(yabs)], -1)
+    return dpi @ dy, dpi @ R, pabs + np.abs(pix)
+
+
+def ba_linearize_terms(poses, points, pix, cidx, pidx, kind=0, delta=1.0):
+    """Sum of |term| of each output of ba_linearize: the stored rows (m,12) / (m,6) and rs (m,2) scaled by sqrt(rho'),
+    Hcc (C,21), Hpp (P,6), gc (C,6), gp (P,3) and the cost."""
+    r = ba_residual(poses, points, pix, cidx, pidx)
+    Jc_abs, Jp_abs, rabs = ba_terms(poses, points, pix, cidx, pidx)
+    rho, w = robust(kind, delta, (r ** 2).sum(-1))
+    ww = w * _weight_factor(kind, delta, rabs)
+    sw = np.sqrt(ww)
+    C, P = poses.shape[0], points.shape[0]
+    iu, iu3 = np.triu_indices(6), np.triu_indices(3)
+    Hcc = _group_sum(cidx, np.einsum('mka,mkb->mab', Jc_abs, Jc_abs)[:, iu[0], iu[1]] * ww[:, None], C)
+    Hpp = _group_sum(pidx, np.einsum('mka,mkb->mab', Jp_abs, Jp_abs)[:, iu3[0], iu3[1]] * ww[:, None], P)
+    gc = _group_sum(cidx, np.einsum('mka,mk->ma', Jc_abs, rabs) * ww[:, None], C)
+    gp = _group_sum(pidx, np.einsum('mka,mk->ma', Jp_abs, rabs) * ww[:, None], P)
+    cost = _rho_terms(kind, delta, (r ** 2).sum(-1)).sum() + (w * 2 * (np.abs(r) * rabs).sum(-1)).sum()
+    return ((Jc_abs * sw[:, None, None]).reshape(-1, 12), (Jp_abs * sw[:, None, None]).reshape(-1, 6), rabs * sw[:, None],
+            Hcc, Hpp, gc, gp, np.array([cost]))
+
+
+def ba_rows_from_y(y, sw, poses, cidx, absolute=False):
+    """Stored BA rows rebuilt from the camera-frame point y and sqrt(rho') (the Y4 layout): Jc (m,2,6), Jp (m,2,3);
+    with absolute=True their magnitudes (y taken as exact)."""
+    m = len(y)
+    z = y[:, 2]
+    dpi = np.zeros((m, 2, 3))
+    dpi[:, 0, 0] = dpi[:, 1, 1] = -1 / z
+    dpi[:, 0, 2], dpi[:, 1, 2] = y[:, 0] / z ** 2, y[:, 1] / z ** 2
+    dy = np.concatenate([np.broadcast_to(np.eye(3), (m, 3, 3)), O.vec2skew(-y)], -1)
+    R = _rot(poses[cidx][:, 3:])
+    if absolute:
+        dpi, dy, R = np.abs(dpi), np.abs(dy), np.abs(R)
+    s = np.abs(sw) if absolute else sw
+    return dpi @ dy * s[:, None, None], dpi @ R * s[:, None, None]
+
+
+# ------------------------------------------------------------------ predicted reductions x^T H x + 2 x^T g for any x
+def pgo_predicted(M21, u, ei, ej, x, terms=False):
+    """x^T H x + 2 x^T g of the pose graph from per-edge blocks: H = sum_e (e_i - e_j) M_e (e_i - e_j)^T, g = pgo_scatter's.
+    terms=True: (value, sum of |term|)."""
+    M = _triu_unpack(M21)
+    d = x[ei] - x[ej]
+    val = np.einsum('ea,eab,eb->', d, M, d) - 2 * (d * u).sum()
+    if not terms:
+        return val
+    da = np.abs(x[ei]) + np.abs(x[ej])
+    return val, np.einsum('ea,eab,eb->', da, np.abs(M), da) + 2 * (da * np.abs(u)).sum()
+
+
+def ba_predicted(Jc, Jp, rs, cidx, pidx, xc, xp, terms=False):
+    """sum_k (J_k x)^T (2 r_k + J_k x), J_k x = Jc_k xc[c_k] + Jp_k xp[p_k] (stored rows, (m,12) / (m,6)).
+    terms=True: (value, sum of |term|)."""
+    Jc, Jp = Jc.reshape(-1, 2, 6), Jp.reshape(-1, 2, 3)
+    Jd = (Jc @ xc[cidx][..., None] + Jp @ xp[pidx][..., None])[..., 0]
+    val = (Jd * (2 * rs + Jd)).sum()
+    if not terms:
+        return val
+    Ja = (np.abs(Jc) @ np.abs(xc[cidx])[..., None] + np.abs(Jp) @ np.abs(xp[pidx])[..., None])[..., 0]
+    return val, (Ja * (2 * np.abs(rs) + Ja)).sum()
+
+
+def node_layout(ei, ej, N):
+    """Node-ordered slots of the edges: edge e owns slot epos_i[e] in node ei[e]'s list and epos_j[e] in ej[e]'s; node n's
+    slots are nptr[n] .. nptr[n+1], in the order of a stable sort of the keys [ei, ej]; nother[s] is the other endpoint."""
+    ei, ej = np.asarray(ei, np.int64), np.asarray(ej, np.int64)
+    E = len(ei)
+    keys = np.concatenate([ei, ej])
+    order = np.argsort(keys, kind="stable")
+    pos = np.empty(2 * E, np.int64)
+    pos[order] = np.arange(2 * E)
+    nptr = np.concatenate([[0], np.cumsum(np.bincount(keys, minlength=N))])
+    nother = np.concatenate([ej, ei])[order]
+    return pos[:E], pos[E:], nptr, nother
