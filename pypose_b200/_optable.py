@@ -387,6 +387,79 @@ LM_OPS += [
 ]
 
 
+# BAL bundle adjustment (csrc/bal.cu): cameras carry [xi (6) | f, k1, k2] unknowns (9), intrinsics (C,3) = (f, k1, k2);
+# observations are grouped by camera as for b200_lm_ba_*_seg.  Model: examples/module/ba/bundle_adjustment.py `Reproj`.
+_BAL_SEG = [("long long", "split", "work items per camera"), ("long long", "tpi", "threads per work item: 32 or 128")]
+LM_OPS += [
+    ("b200_lm_bal_linearize_seg",
+     [("const REAL*", "poses", "(C,7)"), ("const REAL*", "intr", "(C,3) f, k1, k2"), ("const REAL*", "points", "(P,3)"),
+      ("const REAL*", "pix", "(m,2) camera-sorted"), ("const int*", "pidx", "(m) camera-sorted"),
+      ("const int*", "cseg", "(C+1) row offsets per camera"), *_BAL_SEG,
+      ("REAL*", "Y4", "(m,4) y = T p and sqrt(rho')"), ("const int*", "ppos", "(m) position in point order, or NULL"),
+      ("REAL*", "Y4p", "(m,4) point-ordered copy, or NULL"), ("REAL*", "rs", "(m,2) (scaled) residual"),
+      ("REAL*", "Hcc", "(C,45) written"), ("REAL*", "gc", "(C,9) written"), ("REAL*", "part", "(C*split,54) or NULL when split == 1"),
+      ("double*", "ws", "ws[0] = sum rho"), ("int", "robust", ""), ("double", "delta", "")],
+     "modjac + J^T J camera blocks of the BAL model (optimizer.py:645-656), one writer per camera: bit-reproducible"),
+    ("b200_lm_bal_point_blocks",
+     [("const REAL*", "Y4p", "(m,4) point-ordered"), ("const REAL*", "pix_p", "(m,2) point-ordered pixels"),
+      ("const REAL*", "poses", "(C,7)"), ("const REAL*", "intr", "(C,3)"), ("const int*", "cidx_p", "(m)"),
+      ("const int*", "pptr", "(P+1)"), ("REAL*", "Hpp", "(P,6) written"), ("REAL*", "gp", "(P,3) written")],
+     "J^T J / J^T R point blocks of the BAL model by gather (no atomics)"),
+    ("b200_lm_bal_wv_seg",
+     [("const REAL*", "Y4", "(m,4)"), ("const REAL*", "poses", "(C,7)"), ("const REAL*", "intr", "(C,3)"),
+      ("const int*", "pidx", "(m)"), ("const int*", "cseg", "(C+1)"), *_BAL_SEG,
+      ("const REAL*", "Hpinv", "(P,6) or NULL if t holds Hpp^-1 t"), ("const REAL*", "t", "(P,3)"),
+      ("REAL*", "y", "(C,9) y -= W Hpp^-1 t, one writer per camera"), ("REAL*", "part", "(C*split,9) or NULL when split == 1")],
+     "off-diagonal product of the reduced BAL camera system, optim/solver.py:319-336, deterministic"),
+    ("b200_lm_bal_schur_diag_seg",
+     [("const REAL*", "Y4", "(m,4)"), ("const REAL*", "poses", "(C,7)"), ("const REAL*", "intr", "(C,3)"),
+      ("const int*", "pidx", "(m)"), ("const int*", "cseg", "(C+1)"), *_BAL_SEG, ("const REAL*", "Hpinv", "(P,6)"),
+      ("REAL*", "Sd", "(C,45) in: damped Hcc; out: minus sum_k W_k Hpp^-1 W_k^T, one writer per camera"),
+      ("REAL*", "part", "(C*split,45) or NULL when split == 1")],
+     "diagonal blocks of the reduced BAL camera system (preconditioner of the Schur PCG), deterministic"),
+    ("b200_lm_bal_wtx_gather",
+     [("const REAL*", "Y4p", "(m,4) point-ordered"), ("const REAL*", "poses", "(C,7)"), ("const REAL*", "intr", "(C,3)"),
+      ("const int*", "cidx_p", "(m)"), ("const int*", "pptr", "(P+1)"), ("const REAL*", "Hpinv", "(P,6)"),
+      ("const REAL*", "x", "(C,9)"), ("const REAL*", "t0", "(P,3) or NULL"), ("double", "alpha", ""),
+      ("REAL*", "u", "(P,3) alpha * Hpp^-1 (t0 + W^T x), no atomics")],
+     "W^T x of the BAL Schur PCG by gather + the point-block solve; with t0 = gp, alpha = -1 the back-substitution"),
+    ("b200_lm_bal_damp_inv",
+     [("const REAL*", "H", "(n,45) packed 9x9 blocks"), ("double", "scale", "prod(1+damping) over trials"),
+      ("double", "dmin", "diag clamp min"), ("double", "dmax", "diag clamp max"), ("REAL*", "Hd", "(n,45) damped blocks or NULL"),
+      ("REAL*", "Minv", "(n,45) inverses of the damped blocks or NULL")],
+     "clamp + cumulative damping of the diagonal (optimizer.py:657/666) on 9x9 camera blocks"),
+    ("b200_lm_bal_pcg",
+     [("const REAL*", "Y4", "(m,4)"), ("const REAL*", "poses", "(C,7)"), ("const REAL*", "intr", "(C,3)"),
+      ("const int*", "pidx", "(m) camera-sorted"), ("const int*", "cseg", "(C+1)"), *_BAL_SEG, ("long long", "m", "observations"),
+      ("const REAL*", "Y4p", "(m,4)"), ("const int*", "cidx_p", "(m)"), ("const int*", "pptr", "(P+1)"),
+      ("const REAL*", "Hc", "(C,45) damped camera blocks"), ("const REAL*", "Hpinv", "(P,6)"),
+      ("const REAL*", "Minv", "(C,45) preconditioner blocks"), ("const REAL*", "bneg", "(C,9) minus the right-hand side"),
+      ("REAL*", "x", "(C,9) solution"), ("REAL*", "r", "(C,9)"), ("REAL*", "z", "(C,9)"), ("REAL*", "p", "(C,9)"),
+      ("REAL*", "q", "(C,9)"), ("REAL*", "t", "(P,3) work"), ("REAL*", "part", "(C*split,9) or NULL when split == 1"),
+      ("REAL*", "xbest", "(C,9)"), ("double*", "cg", "(16) state, see b200_lm_pgo_pcg"), ("double*", "ws", "reduction workspace"),
+      ("double", "tol", ""), ("long long", "maxiter", ""), ("long long", "P", "points"), ("long long", "first_iter", ""),
+      ("long long", "iters", "")],
+     "PCG on the BAL Schur complement (Hcc - W Hpp^-1 W^T) dc = rhs; optim/solver.py:312-340; no atomics"),
+    ("b200_lm_bal_cg_finish",
+     [("REAL*", "x", "(n,9)"), ("const REAL*", "xbest", "(n,9)"), ("const double*", "cg", "(16) state")],
+     "x <- best iterate unless the PCG converged (the best-iterate guard of b200_lm_cg_finish at width 9)"),
+    ("b200_lm_bal_predicted",
+     [("const REAL*", "Y4", "(m,4)"), ("const REAL*", "poses", "(C,7)"), ("const REAL*", "intr", "(C,3)"),
+      ("const REAL*", "rs", "(m,2)"), ("const int*", "cidx", "(m)"), ("const int*", "pidx", "(m)"),
+      ("const REAL*", "xc", "(C,9)"), ("const REAL*", "xp", "(P,3)"), ("double*", "ws", "ws[0] = sum (J d)^T (2 r + J d)")],
+     "TrustRegion 'predicted' reduction of the BAL model, optim/strategy.py:143"),
+    ("b200_lm_bal_loss",
+     [("const REAL*", "poses", "(C,7)"), ("const REAL*", "intr", "(C,3)"), ("const REAL*", "points", "(P,3)"),
+      ("const REAL*", "pix", "(m,2)"), ("const int*", "cidx", "(m)"), ("const int*", "pidx", "(m)"),
+      ("double*", "ws", "ws[0] = sum rho(|r|^2)"), ("int", "robust", ""), ("double", "delta", "")],
+     "RobustModel.loss of the BAL model, optimizer.py:118-125"),
+    ("b200_lm_bal_retract",
+     [("const REAL*", "poses", "(C,7)"), ("const REAL*", "intr", "(C,3)"), ("const REAL*", "points", "(P,3)"),
+      ("const REAL*", "xc", "(C,9) [xi | dK]"), ("const REAL*", "xp", "(P,3)"), ("REAL*", "poses_t", "(C,7) Exp(xi) T"),
+      ("REAL*", "intr_t", "(C,3) K + dK"), ("REAL*", "points_t", "(P,3) p + dp"), ("long long", "C", "cameras; n = points")],
+     "LM update of the three BAL parameters, lietensor.py:442-444 (poses) and addition (intrinsics, points)"),
+]
+
 def lm_symbols():
     """Yield (symbol, [(ctype, name, comment)], citation)."""
     for base, args, cite in LM_OPS:

@@ -13,32 +13,9 @@
 // Reference semantics: these are the J^T J / J^T R sums of optimizer.py:645-656 (sparse counterpart: bae
 // autograd.graph.jacobian + J.mT @ J, optimizer.py:637-642) for the two-parameter reprojection model README.md:163-198.
 #include "lm_common.cuh"
+#include "lm_seg.cuh"
 
 namespace b200pose {
-
-// fixed-order reduction of NV values over the TPI threads of an item; the result is valid in the item's first thread
-template <typename T, int NV, int TPI>
-__device__ __forceinline__ void item_reduce(T (&v)[NV], T (*sh)[NV]) {
-#pragma unroll
-  for (int k = 0; k < NV; ++k)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-  if (TPI > 32) {                                   // one item per CTA: fold the warp partials in warp order
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    __syncthreads();                                // previous item's readers are done with sh
-    if (lane == 0)
-#pragma unroll
-      for (int k = 0; k < NV; ++k) sh[warp][k] = v[k];
-    __syncthreads();
-    if (threadIdx.x == 0)
-#pragma unroll
-      for (int k = 0; k < NV; ++k) {
-        T t = sh[0][k];
-        for (int w = 1; w < TPI / 32; ++w) t += sh[w][k];
-        v[k] = t;
-      }
-  }
-}
 
 // rows of one observation from y (camera frame), the robust scale and the camera quaternion (held by the item)
 template <typename T>
@@ -51,17 +28,6 @@ __device__ __forceinline__ void rows_from_y(const V3<T>& y, T sw, const Q4<T>& q
   for (int a = 0; a < 6; ++a) { R.jc0[a] *= sw; R.jc1[a] *= sw; }
 #pragma unroll
   for (int a = 0; a < 3; ++a) { R.jp0[a] *= sw; R.jp1[a] *= sw; }
-}
-
-struct ItemRange { long long c; int b, e; };
-__device__ __forceinline__ ItemRange item_range(long long it, int S, const int* __restrict__ cseg) {
-  ItemRange r;
-  r.c = it / S;
-  const int s = (int)(it - r.c * S);
-  const long long b = cseg[r.c], len = (long long)cseg[r.c + 1] - b;
-  r.b = (int)(b + len * s / S);
-  r.e = (int)(b + len * (s + 1) / S);
-  return r;
 }
 
 // Linearisation: per observation y = T_c p_j, residual, robust scale; stores Y4 (camera order), Y4p (point order) and the
@@ -134,23 +100,6 @@ __global__ void __launch_bounds__(kLmThreads) ba_linearize_seg_kernel(
     }
   }
   reduce_sums<1>(acc, ws);
-}
-
-// dst (+)= sum_s part[(c, s)] in s order; the first WA values go to A (stride WA), the remaining WB to B (stride WB)
-template <typename T>
-__global__ void __launch_bounds__(kLmThreads) cam_fold_kernel(const T* __restrict__ part, int S, int WA, int WB,
-                                                               T* __restrict__ A, T* __restrict__ B, int add,
-                                                               const double* cg, long long C) {
-  if (cg && cg[5] != 0.0) return;
-  const int NV = WA + WB;
-  for (long long i = (long long)blockIdx.x * kLmThreads + threadIdx.x; i < C * NV; i += (long long)gridDim.x * kLmThreads) {
-    const long long c = i / NV;
-    const int v = (int)(i - c * NV);
-    T t = T(0);
-    for (int s = 0; s < S; ++s) t += part[(c * S + s) * NV + v];
-    T* d = v < WA ? A + c * WA + v : B + c * WB + (v - WA);
-    *d = add ? *d + t : t;
-  }
 }
 
 // Point blocks Hpp (6) and gp (3) by gather over the point-ordered rows: LPP lanes per point, fixed shuffle tree.
@@ -318,11 +267,6 @@ __global__ void __launch_bounds__(kLmThreads) ba_schur_diag_seg_kernel(const T* 
       }
     }
   }
-}
-
-static inline unsigned item_grid(long long items, int tpi) {
-  const int ipb = kLmThreads / tpi;
-  return lm_grid(items, ipb);
 }
 
 template <typename CT>

@@ -12,60 +12,10 @@
 // Reductions are the deterministic last-block fp64 folds of lm_common.cuh.
 #include "lm_common.cuh"
 #include "comm.cuh"
+#include "pcg_vec.cuh"
 
 namespace b200pose {
 
-// state (16 doubles).  DONE: 0 running, 1 converged (|r| <= tol |b|), 2 breakdown (p.Ap <= 0), 3 stagnated (no new minimum of
-// |r| for PATIENCE = max(100, unknowns) iterations), 4 maxiter.  BEST / SINCE / SAVE guard the solve against finite-precision CG: when the
-// tolerance is below what the arithmetic can reach (fp32, ill-conditioned Schur complements) the iterate degrades after
-// its best point, so the iterate with the smallest recursive residual is kept in xbest and returned unless the solve
-// converged (then the last iterate IS the best one, i.e. attainable tolerances behave exactly like solver.py:312-340).
-enum { CG_RZ0 = 0, CG_RZ1 = 1, CG_PQ = 2, CG_RR = 3, CG_STOP2 = 4, CG_DONE = 5, CG_ITERS = 6, CG_MAXIT = 7,
-       CG_BEST = 8, CG_SINCE = 9, CG_SAVE = 10, CG_PATIENCE = 11, CG_STATE = 16 };
-constexpr double kCgPatience = 100.0;
-
-// after an update produced |r|^2 = rr: bookkeeping of the best iterate and the stop decision (one thread)
-__device__ __forceinline__ void cg_after_update(double* cg, double rr, double it) {
-  if (rr < cg[CG_BEST]) { cg[CG_BEST] = rr; cg[CG_SINCE] = 0.0; cg[CG_SAVE] = 1.0; }
-  else { cg[CG_SINCE] += 1.0; cg[CG_SAVE] = 0.0; }
-  if (!(rr > cg[CG_STOP2])) cg[CG_DONE] = 1.0;
-  else if (it >= cg[CG_MAXIT]) cg[CG_DONE] = 4.0;
-  else if (cg[CG_SINCE] >= cg[CG_PATIENCE]) cg[CG_DONE] = 3.0;
-}
-
-// (n, 6) vectors are read and written as three 8-byte (float) / 16-byte (double) pairs: a node's six values start at a
-// multiple of 24 / 48 bytes, so the arrays only have to be 8- / 16-byte aligned (checked at the entry points).  Scalar
-// accesses cost one LSU wavefront per touched line and instruction — 36 per warp and vector instead of 18 (the PCG
-// kernels are LSU-bound, not DRAM-bound).
-template <typename T> struct Pair6;
-template <> struct Pair6<float> { using type = float2; };
-template <> struct Pair6<double> { using type = double2; };
-template <typename T> __device__ __forceinline__ void ld6(const T* p, long long i, T (&v)[6]) {
-  using P = typename Pair6<T>::type;
-  const P* q = reinterpret_cast<const P*>(p + i * 6);
-#pragma unroll
-  for (int k = 0; k < 3; ++k) { const P t = q[k]; v[2 * k] = t.x; v[2 * k + 1] = t.y; }
-}
-template <typename T> __device__ __forceinline__ void st6(T* p, long long i, const T (&v)[6]) {
-  using P = typename Pair6<T>::type;
-  P* q = reinterpret_cast<P*>(p + i * 6);
-#pragma unroll
-  for (int k = 0; k < 3; ++k) { P t; t.x = v[2 * k]; t.y = v[2 * k + 1]; q[k] = t; }
-}
-template <typename T> __device__ __forceinline__ void sym6_mv_packed(const T* a21, const T (&x)[6], T (&y)[6]) {
-  T A[6][6];
-  sym6_unpack(a21, A);
-  sym6_mv(A, x, y);
-}
-// q = D p with D none (0), diagonal (n,6) (1) or packed symmetric blocks (n,21) (2)
-template <typename T> __device__ __forceinline__ void apply_D(const T* D, int dmode, long long i, const T (&p)[6], T (&q)[6]) {
-  if (dmode == 2) {
-    sym6_mv_packed(D + i * 21, p, q);
-  } else {
-#pragma unroll
-    for (int k = 0; k < 6; ++k) q[k] = dmode == 1 ? D[i * 6 + k] * p[k] : T(0);
-  }
-}
 
 // diag <- clamp(diag, dmin, dmax) * scale (optimizer.py:657 + cumulative :666); optional outputs: the damped block,
 // the amount added to the diagonal, the inverse of the damped block.
@@ -86,233 +36,6 @@ __global__ void __launch_bounds__(kLmThreads) blk6_damp_inv_kernel(const T* __re
     if (Hd) sym6_pack(A, Hd + i * 21);
     if (Minv) { spd_inverse<T, 6>(A, Ai); sym6_pack(Ai, Minv + i * 21); }
   }
-}
-template <typename T>
-__global__ void __launch_bounds__(kLmThreads) pt3_damp_inv_kernel(const T* __restrict__ H, T scale, T dmin, T dmax,
-                                                                   T* __restrict__ Hinv, long long n) {
-  for (long long i = (long long)blockIdx.x * kLmThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kLmThreads) {
-    T A[3][3], Ai[3][3];
-    sym3_unpack(H + i * 6, A);
-#pragma unroll
-    for (int k = 0; k < 3; ++k) { const T d = A[k][k]; A[k][k] = (d < dmin ? dmin : (d > dmax ? dmax : d)) * scale; }
-    spd_inverse<T, 3>(A, Ai);
-    T* o = Hinv + i * 6;
-    o[0] = Ai[0][0]; o[1] = Ai[0][1]; o[2] = Ai[0][2]; o[3] = Ai[1][1]; o[4] = Ai[1][2]; o[5] = Ai[2][2];
-  }
-}
-// out = alpha * A t for packed 3x3 blocks
-template <typename T>
-__global__ void __launch_bounds__(kLmThreads) pt3_apply_kernel(const T* __restrict__ A6, const T* __restrict__ t, T alpha,
-                                                                T* __restrict__ out, long long n) {
-  for (long long i = (long long)blockIdx.x * kLmThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kLmThreads) {
-    T A[3][3];
-    sym3_unpack(A6 + i * 6, A);
-    const T a = t[i * 3], b = t[i * 3 + 1], c = t[i * 3 + 2];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) out[i * 3 + k] = alpha * (A[k][0] * a + A[k][1] * b + A[k][2] * c);
-  }
-}
-
-// ---- CG vector kernels -------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(kLmThreads) cg_init_kernel(const T* __restrict__ Minv, const T* __restrict__ b, T sign,
-                                                              const T* __restrict__ D, int dmode, T* __restrict__ x,
-                                                              T* __restrict__ r, T* __restrict__ p, T* __restrict__ q,
-                                                              double* cg, double* ws, double tol, double maxiter,
-                                                              long long n) {
-  double acc[2] = {0.0, 0.0};
-  for (long long i = (long long)blockIdx.x * kLmThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kLmThreads) {
-    T rv[6], z[6], qv[6], zero[6] = {T(0), T(0), T(0), T(0), T(0), T(0)};
-    ld6(b, i, rv);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) rv[k] *= sign;
-    sym6_mv_packed(Minv + i * 21, rv, z);
-    apply_D(D, dmode, i, z, qv);
-    st6(x, i, zero); st6(r, i, rv); st6(p, i, z); st6(q, i, qv);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) { acc[0] += (double)rv[k] * (double)z[k]; acc[1] += (double)rv[k] * (double)rv[k]; }
-  }
-  if (reduce_sums<2>(acc, ws)) {
-    const double rz = ws[0], rr = ws[1];
-    cg[CG_RZ0] = rz; cg[CG_RZ1] = 0.0; cg[CG_PQ] = 0.0; cg[CG_RR] = rr; cg[CG_STOP2] = tol * tol * rr;
-    cg[CG_ITERS] = 0.0; cg[CG_MAXIT] = maxiter;
-    cg[CG_BEST] = rr; cg[CG_SINCE] = 0.0; cg[CG_SAVE] = 1.0;       // x = 0 is the first best
-    // exact CG ends within (number of unknowns) iterations: no new minimum of |r| for that long is stagnation, not a plateau
-    cg[CG_PATIENCE] = fmax(kCgPatience, 6.0 * (double)n);
-    cg[CG_DONE] = (!(rr > tol * tol * rr) || maxiter <= 0.0) ? 1.0 : 0.0;      // |r| <= tol |b| (also NaN) -> nothing to do
-  }
-}
-template <typename T>
-__global__ void __launch_bounds__(kLmThreads) cg_dot_kernel(const T* __restrict__ p, const T* __restrict__ q, double* cg,
-                                                             double* ws, long long n) {
-  if (cg[CG_DONE] != 0.0) return;
-  double acc[1] = {0.0};
-  for (long long i = (long long)blockIdx.x * kLmThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kLmThreads) {
-#pragma unroll
-    for (int k = 0; k < 6; ++k) acc[0] += (double)p[i * 6 + k] * (double)q[i * 6 + k];
-  }
-  if (reduce_sums<1>(acc, ws)) cg[CG_PQ] = ws[0];
-}
-template <typename T>
-__global__ void __launch_bounds__(kLmThreads) cg_update_kernel(const T* __restrict__ Minv, const T* __restrict__ p,
-                                                                const T* __restrict__ q, T* __restrict__ x,
-                                                                T* __restrict__ r, T* __restrict__ z,
-                                                                T* __restrict__ xbest, double* cg,
-                                                                double* ws, int par, long long n) {
-  if (cg[CG_DONE] != 0.0) return;
-  const bool save = cg[CG_SAVE] != 0.0;      // the iterate entering this update is the best so far: keep a copy
-  const double pq = cg[CG_PQ];
-  if (!(pq > 0.0)) {                       // breakdown (operator not positive definite along p): stop with the current x
-    if (blockIdx.x == 0 && threadIdx.x == 0) cg[CG_DONE] = 2.0;
-    return;
-  }
-  const T alpha = (T)(cg[par] / pq);
-  double acc[2] = {0.0, 0.0};
-  // The 21-word preconditioner blocks of a warp's 32 consecutive nodes are 2688 contiguous bytes: the warp copies them
-  // with 21 coalesced loads into shared memory (one wavefront each) and every lane reads its block from there (stride 21
-  // words: conflict-free) — read per lane straight from global memory, each of the 21 load instructions touched 21 lines.
-  __shared__ T sM[kLmThreads / 32][32 * 21];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (long long base = (long long)blockIdx.x * kLmThreads + warp * 32; base < n; base += (long long)gridDim.x * kLmThreads) {
-    const long long i = base + lane;
-    const int words = (int)(n - base < 32 ? n - base : 32) * 21;
-    __syncwarp();
-    for (int w = lane; w < words; w += 32) sM[warp][w] = Minv[base * 21 + w];
-    __syncwarp();
-    if (i >= n) continue;
-    T pv[6], qv[6], xv[6], rv[6], zv[6];
-    ld6(p, i, pv); ld6(q, i, qv); ld6(x, i, xv); ld6(r, i, rv);
-    if (save) st6(xbest, i, xv);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) { xv[k] += alpha * pv[k]; rv[k] -= alpha * qv[k]; }
-    sym6_mv_packed(&sM[warp][lane * 21], rv, zv);
-    st6(x, i, xv); st6(r, i, rv); st6(z, i, zv);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) { acc[0] += (double)rv[k] * (double)zv[k]; acc[1] += (double)rv[k] * (double)rv[k]; }
-  }
-  if (reduce_sums<2>(acc, ws)) {       // thread 0 of the last CTA: every CTA has read the state it needs by now
-    cg[par ^ 1] = ws[0];
-    cg[CG_RR] = ws[1];
-    const double it = cg[CG_ITERS] + 1.0;
-    cg[CG_ITERS] = it;
-    cg_after_update(cg, ws[1], it);
-  }
-}
-// x <- xbest unless the solve converged or the last iterate is the best one (see the state enum)
-template <typename T>
-__global__ void __launch_bounds__(kLmThreads) cg_finish_kernel(T* __restrict__ x, const T* __restrict__ xbest,
-                                                                const double* cg, long long n6) {
-  if (cg[CG_DONE] == 1.0 || cg[CG_SAVE] != 0.0) return;
-  for (long long i = (long long)blockIdx.x * kLmThreads + threadIdx.x; i < n6; i += (long long)gridDim.x * kLmThreads)
-    x[i] = xbest[i];
-}
-template <typename T>
-__global__ void __launch_bounds__(kLmThreads) cg_dir_kernel(const T* __restrict__ z, const T* __restrict__ D, int dmode,
-                                                             T* __restrict__ p, T* __restrict__ q, const double* cg, int par,
-                                                             long long n) {
-  if (cg[CG_DONE] != 0.0) return;
-  const T beta = (T)(cg[par ^ 1] / cg[par]);
-  for (long long i = (long long)blockIdx.x * kLmThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kLmThreads) {
-    T pv[6], zv[6], qv[6];
-    ld6(p, i, pv); ld6(z, i, zv);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) pv[k] = zv[k] + beta * pv[k];
-    apply_D(D, dmode, i, pv, qv);
-    st6(p, i, pv); st6(q, i, qv);
-  }
-}
-
-// dot + update + dir of one iteration in ONE single-CTA launch, for systems small enough that a grid is only latency
-// (bundle adjustment: a few thousand cameras; the three separate kernels cost ~28 us at 1e3 rows, this one ~8 us).
-// Fixed-order block reductions (warp shuffles, then warp 0 over the 32 warp partials): deterministic.
-constexpr long long kVecSmallRows = 4096;
-template <int NS, int THREADS> __device__ __forceinline__ void block_sums(double (&v)[NS], double (*sh)[NS], double (&out)[NS]) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < NS; ++k)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-  if (lane == 0)
-#pragma unroll
-    for (int k = 0; k < NS; ++k) sh[warp][k] = v[k];
-  __syncthreads();
-  if (warp == 0) {
-    double t[NS];
-#pragma unroll
-    for (int k = 0; k < NS; ++k) {
-      t[k] = lane < THREADS / 32 ? sh[lane][k] : 0.0;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) t[k] += __shfl_xor_sync(0xffffffffu, t[k], o);
-    }
-    if (lane == 0)
-#pragma unroll
-      for (int k = 0; k < NS; ++k) sh[0][k] = t[k];
-  }
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < NS; ++k) out[k] = sh[0][k];
-  __syncthreads();
-}
-template <typename T, int THREADS>
-__global__ void __launch_bounds__(THREADS) cg_vec_small_kernel(const T* __restrict__ Minv, const T* __restrict__ D, int dmode,
-                                                                    T* __restrict__ x, T* __restrict__ r, T* __restrict__ z,
-                                                                    T* __restrict__ p, T* __restrict__ q,
-                                                                    T* __restrict__ xbest, double* cg, int par,
-                                                                    long long n) {
-  __shared__ double sh[32][2];
-  __shared__ double done_sh;
-  if (cg[CG_DONE] != 0.0) return;
-  const double rz_old = cg[par], it = cg[CG_ITERS] + 1.0;
-  const bool save = cg[CG_SAVE] != 0.0;
-  double a1[2] = {0.0, 0.0}, s1[2];
-  for (long long i = threadIdx.x; i < n; i += THREADS)
-#pragma unroll
-    for (int k = 0; k < 6; ++k) a1[0] += (double)p[i * 6 + k] * (double)q[i * 6 + k];
-  block_sums<2, THREADS>(a1, sh, s1);
-  const double pq = s1[0];
-  if (!(pq > 0.0)) {                       // breakdown: stop with the current x
-    if (threadIdx.x == 0) cg[CG_DONE] = 2.0;
-    return;
-  }
-  const T alpha = (T)(rz_old / pq);
-  double a2[2] = {0.0, 0.0}, s2[2];
-  for (long long i = threadIdx.x; i < n; i += THREADS) {
-    T pv[6], qv[6], xv[6], rv[6], zv[6];
-    ld6(p, i, pv); ld6(q, i, qv); ld6(x, i, xv); ld6(r, i, rv);
-    if (save) st6(xbest, i, xv);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) { xv[k] += alpha * pv[k]; rv[k] -= alpha * qv[k]; }
-    sym6_mv_packed(Minv + i * 21, rv, zv);
-    st6(x, i, xv); st6(r, i, rv); st6(z, i, zv);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) { a2[0] += (double)rv[k] * (double)zv[k]; a2[1] += (double)rv[k] * (double)rv[k]; }
-  }
-  block_sums<2, THREADS>(a2, sh, s2);
-  if (threadIdx.x == 0) {
-    cg[CG_PQ] = pq; cg[par ^ 1] = s2[0]; cg[CG_RR] = s2[1]; cg[CG_ITERS] = it;
-    cg_after_update(cg, s2[1], it);
-    done_sh = cg[CG_DONE];
-  }
-  __syncthreads();
-  if (done_sh != 0.0) return;
-  const T beta = (T)(s2[0] / rz_old);
-  for (long long i = threadIdx.x; i < n; i += THREADS) {     // the same thread wrote z[i] above
-    T pv[6], zv[6], qv[6];
-    ld6(p, i, pv); ld6(z, i, zv);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) pv[k] = zv[k] + beta * pv[k];
-    apply_D(D, dmode, i, pv, qv);
-    st6(p, i, pv); st6(q, i, qv);
-  }
-}
-
-template <typename T>
-static void launch_cg_vec_small(const T* Minv, const T* D, int dmode, T* x, T* r, T* z, T* p, T* q, T* xbest, double* cg,
-                                int par, long long n, cudaStream_t st) {
-  const int th = n <= 2048 ? 256 : (n <= 3072 ? 512 : 1024);     // measured: 256 beats 1024 at 1e3 rows
-  if (th == 256) cg_vec_small_kernel<T, 256><<<1, 256, 0, st>>>(Minv, D, dmode, x, r, z, p, q, xbest, cg, par, n);
-  else if (th == 512) cg_vec_small_kernel<T, 512><<<1, 512, 0, st>>>(Minv, D, dmode, x, r, z, p, q, xbest, cg, par, n);
-  else cg_vec_small_kernel<T, 1024><<<1, 1024, 0, st>>>(Minv, D, dmode, x, r, z, p, q, xbest, cg, par, n);
 }
 
 // ---- operators (ObsRows / obs_rows: lm_common.cuh) -----------------------------------------------------------------

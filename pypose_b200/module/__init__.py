@@ -1,6 +1,6 @@
 from .reproj import PoseReproj, TwoPoseReproj
 from .pgo import PoseGraph
-from .ba import BundleAdjustment
+from .ba import BundleAdjustment, BALBundleAdjustment
 from .imu_preintegrator import IMUPreintegrator
 from .loss import GeodesicLoss, geodesic_loss
 from .pnp import EPnP

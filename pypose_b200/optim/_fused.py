@@ -459,6 +459,77 @@ def ba_solve(Y4s, poses, rs, cidx, pidx, geom, Hcc, Hpp, gc, gp, scale, dmin, dm
     return x, xp, iters, ws[:1].clone()
 
 
+def bal_linearize(intr, poses, points, pix, pidx, geom, robust=0, delta=1.0):
+    """BAL linearisation (csrc/bal.cu): Y4 / Y4p / rs per observation, 9x9 camera blocks Hcc (C,45) and gc (C,9) with one
+    writer per camera, point blocks Hpp (P,6) and gp (P,3) by gather.  `geom` as for ba_linearize_det (BALProblem)."""
+    cseg, split, tpi, ppos, cidx_p, pptr, pix_p = geom
+    intr, poses, points, pix = _same(intr, poses, points, pix)
+    m, C, P = pix.shape[0], poses.shape[0], points.shape[0]
+    dt, dev = poses.dtype, poses.device
+    ws = _workspace(dev)
+    Y4, Y4p, rs = (torch.empty(m, w, dtype=dt, device=dev) for w in (4, 4, 2))
+    Hcc, gc = torch.empty(C, 45, dtype=dt, device=dev), torch.empty(C, 9, dtype=dt, device=dev)
+    Hpp, gp = torch.empty(P, 6, dtype=dt, device=dev), torch.empty(P, 3, dtype=dt, device=dev)
+    part = torch.empty(C * split, 54, dtype=dt, device=dev) if split > 1 else None
+    _launch("b200_lm_bal_linearize_seg", poses, [_p(poses), _p(intr), _p(points), _p(pix), _p(pidx), _p(cseg), split, tpi,
+                                                 _p(Y4), _p(ppos), _p(Y4p), _p(rs), _p(Hcc), _p(gc), _p(part), _p(ws),
+                                                 int(robust), float(delta)], C)
+    cur = ws[:1].clone()
+    _launch("b200_lm_bal_point_blocks", poses, [_p(Y4p), _p(pix_p), _p(poses), _p(intr), _p(cidx_p), _p(pptr), _p(Hpp),
+                                                _p(gp)], P)
+    return (Y4, Y4p), rs, Hcc, Hpp, gc, gp, cur
+
+
+def bal_solve(Y4s, intr, poses, rs, cidx, pidx, geom, Hcc, Hpp, gc, gp, scale, dmin, dmax, tol, maxiter, hint=0):
+    """Schur-complement solve of the damped BAL normal equations by device PCG over the 9 unknowns of every camera
+    (csrc/bal.cu); rows are rebuilt from Y4 and the intrinsics / poses of the linearisation.  Returns xc (C,9) =
+    [xi | df, dk1, dk2], xp (P,3), iterations, predicted (1,) fp64 on device."""
+    Y4, Y4p = Y4s
+    cseg, split, tpi, _, cidx_p, pptr, _ = geom
+    dev, dt = Y4.device, Y4.dtype
+    m, C, P = Y4.shape[0], Hcc.shape[0], Hpp.shape[0]
+    ws, cg = _workspace(dev), _cg(dev)
+    Hc, Minv = torch.empty(C, 45, dtype=dt, device=dev), torch.empty(C, 45, dtype=dt, device=dev)
+    Hpinv = torch.empty(P, 6, dtype=dt, device=dev)
+    part = torch.empty(C * split, 45, dtype=dt, device=dev) if split > 1 else None
+    y4, tp, kp, pi_, cs = _p(Y4), _p(poses), _p(intr), _p(pidx), _p(cseg)
+    _launch("b200_lm_bal_damp_inv", Y4, [_p(Hcc), float(scale), float(dmin), float(dmax), _p(Hc), _p(None)], C)
+    _launch("b200_lm_pt3_damp_inv", Y4, [_p(Hpp), float(scale), float(dmin), float(dmax), _p(Hpinv)], P)
+    Sd = Hc.clone()
+    _launch("b200_lm_bal_schur_diag_seg", Y4, [y4, tp, kp, pi_, cs, split, tpi, _p(Hpinv), _p(Sd), _p(part)], C)
+    bneg = gc.clone()                                     # -(rhs) = gc - W Hpp^-1 gp
+    _launch("b200_lm_bal_wv_seg", Y4, [y4, tp, kp, pi_, cs, split, tpi, _p(Hpinv), _p(gp), _p(bneg), _p(part)], C)
+    _launch("b200_lm_bal_damp_inv", Y4, [_p(Sd), 1.0, -3.0e38, 3.0e38, _p(None), _p(Minv)], C)
+    x, r, z, p, q, xbest = (torch.empty(C, 9, dtype=dt, device=dev) for _ in range(6))
+    t = torch.empty(P, 3, dtype=dt, device=dev)
+    maxiter = int(maxiter) if maxiter is not None else 10 * 9 * C
+    iters = _run_chunks(lambda it0, k: _launch("b200_lm_bal_pcg", Y4, [
+        y4, tp, kp, pi_, cs, split, tpi, m, _p(Y4p), _p(cidx_p), _p(pptr), _p(Hc), _p(Hpinv), _p(Minv), _p(bneg), _p(x), _p(r), _p(z), _p(p), _p(q),
+        _p(t), _p(part), _p(xbest), _p(cg), _p(ws), float(tol), maxiter, P, it0, k], C), cg, maxiter, hint)
+    _launch("b200_lm_bal_cg_finish", Y4, [_p(x), _p(xbest), _p(cg)], C)     # best iterate unless the solve converged
+    xp = torch.empty(P, 3, dtype=dt, device=dev)          # dp = -Hpp^-1 (gp + W^T dc)
+    _launch("b200_lm_bal_wtx_gather", Y4, [_p(Y4p), _p(poses), _p(intr), _p(cidx_p), _p(pptr), _p(Hpinv), _p(x), _p(gp),
+                                           -1.0, _p(xp)], P)
+    _launch("b200_lm_bal_predicted", Y4, [_p(Y4), _p(poses), _p(intr), _p(rs), _p(cidx), _p(pidx), _p(x), _p(xp), _p(ws)], m)
+    return x, xp, iters, ws[:1].clone()
+
+
+def bal_loss(intr, poses, points, pix, cidx, pidx, robust=0, delta=1.0):
+    """(1,) fp64 device tensor: sum rho(|r|^2) of the BAL model at the given parameters."""
+    ws = _workspace(poses.device)
+    _launch("b200_lm_bal_loss", poses, [_p(poses), _p(intr), _p(points), _p(pix), _p(cidx), _p(pidx), _p(ws), int(robust),
+                                        float(delta)], pix.shape[0])
+    return ws[:1].clone()
+
+
+def bal_retract(intr, poses, points, xc, xp):
+    """Trial parameters: (K + dK, Exp(xi) T, p + dp) from xc (C,9) = [xi | dK] and xp (P,3)."""
+    Kt, Tt, pt = torch.empty_like(intr), torch.empty_like(poses), torch.empty_like(points)
+    _launch("b200_lm_bal_retract", poses, [_p(poses), _p(intr), _p(points), _p(xc), _p(xp), _p(Tt), _p(Kt), _p(pt),
+                                           poses.shape[0]], points.shape[0])
+    return Kt, Tt, pt
+
+
 # ----------------------------------------------------------------------------------------------------
 # Reprojection LM trial with the fewest host operations (the step is host-bound: ~30 us of kernels, see
 # tools/prof_lm_host.py): outputs are caller-owned buffers, the three kernels reduce into three workspace

@@ -476,6 +476,34 @@ def _unpack6(Hp):
     return A
 
 
+def _group_by_camera(prob, pix, cidx, pidx, C, P):
+    """Observation layout of the deterministic bundle-adjustment routes (csrc/ba.cu, csrc/bal.cu), set on `prob`."""
+    # observations are regrouped by camera once (the LM sums do not depend on their order): the camera-side
+    # scatter-adds of the kernels then collapse to one atomic per warp and value (csrc/lm_common.cuh seg_atomic_add)
+    order = torch.sort(cidx.reshape(-1), stable=True)[1]
+    pix, cidx, pidx = pix.reshape(-1, 2)[order], cidx.reshape(-1)[order], pidx.reshape(-1)[order]
+    prob.pix = pix.to(prob.dtype).contiguous()
+    prob.cidx, prob.pidx = cidx.to(torch.int32).contiguous(), pidx.to(torch.int32).contiguous()
+    prob.cl, prob.pl = cidx.long(), pidx.long()
+    # observation ids grouped by point (CSR): W^T x of the device PCG gathers along it instead of scatter-adding
+    prob.padj = torch.sort(prob.pl, stable=True)[1].contiguous()
+    prob.cidx_p = prob.cidx[prob.padj].contiguous()
+    prob.ppos = torch.empty_like(prob.padj, dtype=torch.int32)          # inverse permutation: position in point order
+    prob.ppos[prob.padj] = torch.arange(prob.padj.numel(), dtype=torch.int32, device=prob.padj.device)
+    prob.pptr = torch.zeros(P + 1, dtype=torch.int32, device=prob.pl.device)
+    prob.pptr[1:] = torch.cumsum(torch.bincount(prob.pl, minlength=P), 0).to(torch.int32)
+    # geometry of the deterministic device route (csrc/ba.cu): rows per camera, work items per camera (so that a few
+    # cameras with very many rows still fill the machine) and threads per item, point-ordered pixels
+    m = prob.cidx.numel()
+    prob.cseg = torch.zeros(C + 1, dtype=torch.int32, device=prob.pl.device)
+    prob.cseg[1:] = torch.cumsum(torch.bincount(prob.cl, minlength=C), 0).to(torch.int32)
+    tpi = 128 if m >= 192 * C else 32
+    sms = _sms(prob.pl.device) if prob.pl.is_cuda else 132     # the geometry only steers the device kernels
+    want = sms * 8 * (128 // tpi)                      # items that fill the SMs
+    split = max(1, min(want // max(C, 1), (m // max(C, 1)) // (8 * tpi))) if C < want else 1
+    prob.geom = (prob.cseg, int(split), int(tpi), prob.ppos, prob.cidx_p, prob.pptr, prob.pix[prob.padj].contiguous())
+
+
 class BAProblem(_Problem):
     """Bundle adjustment with poses (C,7) and points (P,3) as parameters, in the reference's parameter order.
 
@@ -489,31 +517,8 @@ class BAProblem(_Problem):
         self.model, self.key, self.group, self.robust = model, key, group, robust
         self.poses, self.points = (model.poses, model.points_3d) if params is None else params
         self.dtype = self.poses.dtype
-        # observations are regrouped by camera once (the LM sums do not depend on their order): the camera-side
-        # scatter-adds of the kernels then collapse to one atomic per warp and value (csrc/lm_common.cuh seg_atomic_add)
-        order = torch.sort(cidx.reshape(-1), stable=True)[1]
-        pix, cidx, pidx = pix.reshape(-1, 2)[order], cidx.reshape(-1)[order], pidx.reshape(-1)[order]
-        self.pix = pix.to(self.dtype).contiguous()
-        self.cidx, self.pidx = cidx.to(torch.int32).contiguous(), pidx.to(torch.int32).contiguous()
-        self.cl, self.pl = cidx.long(), pidx.long()
-        # observation ids grouped by point (CSR): W^T x of the device PCG gathers along it instead of scatter-adding
-        P = self.points.reshape(-1, 3).shape[0]
-        self.padj = torch.sort(self.pl, stable=True)[1].contiguous()
-        self.cidx_p = self.cidx[self.padj].contiguous()
-        self.ppos = torch.empty_like(self.padj, dtype=torch.int32)          # inverse permutation: position in point order
-        self.ppos[self.padj] = torch.arange(self.padj.numel(), dtype=torch.int32, device=self.padj.device)
-        self.pptr = torch.zeros(P + 1, dtype=torch.int32, device=self.pl.device)
-        self.pptr[1:] = torch.cumsum(torch.bincount(self.pl, minlength=P), 0).to(torch.int32)
-        # geometry of the deterministic device route (csrc/ba.cu): rows per camera, work items per camera (so that a few
-        # cameras with very many rows still fill the machine) and threads per item, point-ordered pixels
-        C, m = self.poses.tensor().reshape(-1, 7).shape[0], self.cidx.numel()
-        self.cseg = torch.zeros(C + 1, dtype=torch.int32, device=self.pl.device)
-        self.cseg[1:] = torch.cumsum(torch.bincount(self.cl, minlength=C), 0).to(torch.int32)
-        tpi = 128 if m >= 192 * C else 32
-        sms = _sms(self.pl.device) if self.pl.is_cuda else 132     # the geometry only steers the device kernels
-        want = sms * 8 * (128 // tpi)                      # items that fill the SMs
-        split = max(1, min(want // max(C, 1), (m // max(C, 1)) // (8 * tpi))) if C < want else 1
-        self.geom = (self.cseg, int(split), int(tpi), self.ppos, self.cidx_p, self.pptr, self.pix[self.padj].contiguous())
+        C, P = self.poses.tensor().reshape(-1, 7).shape[0], self.points.reshape(-1, 3).shape[0]
+        _group_by_camera(self, pix, cidx, pidx, C, P)
         self.tol, self.maxiter = tol, maxiter
         self._trial = None
         self.cg_iters = 0
@@ -630,6 +635,57 @@ class BAProblem(_Problem):
         return ds.trial(self, T, p, scale, dmin, dmax, retry)
 
 
+class BALProblem(_Problem):
+    """BAL bundle adjustment (module.BALBundleAdjustment, the reference's examples/module/ba `Reproj(K, C, P)`): per-camera
+    intrinsics (C,3) = (f, k1, k2), poses (C,7) and points (P,3).  The unknowns of a camera are [xi | f, k1, k2] (9), of
+    a point dp (3); J^T J over all of them is clamped and damped like the dense branch (optimizer.py:657/666) and solved by
+    eliminating the 3x3 point blocks, as BAProblem does, with a device PCG over 9-wide camera blocks (csrc/bal.cu, no
+    atomics).  The update is Exp(xi) T for the poses and addition for intrinsics and points.  One CUDA device, no
+    process group, no residual weights."""
+
+    def __init__(self, model, pix, cidx, pidx, key, robust, tol, maxiter, params):
+        self.model, self.key, self.group, self.robust = model, key, None, robust
+        self.intr, self.poses, self.points = params
+        self.dtype = self.poses.dtype
+        _group_by_camera(self, pix, cidx, pidx, self.poses.shape[0], self.points.shape[0])
+        self.tol, self.maxiter = tol, maxiter
+        self._trial = None
+        self.cg_iters = 0
+
+    def matches(self, model, input, weight=None):
+        return weight is None and model is self.model and _input_key(input) == self.key
+
+    def _params(self):
+        return self.intr.reshape(-1, 3), self.poses.tensor().reshape(-1, 7), self.points.reshape(-1, 3)
+
+    def loss(self):
+        K, T, p = self._params()
+        return _fused.bal_loss(K, T, p, self.pix, self.cidx, self.pidx, *self.robust)[0].to(self.dtype)
+
+    def linearize(self):
+        K, T, p = self._params()
+        return _fused.bal_linearize(K, T, p, self.pix, self.pidx, self.geom, *self.robust)
+
+    def trial(self, lin, scale, dmin, dmax):
+        Y4s, rs, Hcc, Hpp, gc, gp, cur = lin
+        K, T, p = self._params()
+        xc, xp, self.cg_iters, pred = _fused.bal_solve(Y4s, K, T, rs, self.cidx, self.pidx, self.geom, Hcc, Hpp, gc, gp,
+                                                       scale, dmin, dmax, self.tol, self.maxiter,
+                                                       hint=self.cg_iters + 1 if self.cg_iters else 0)
+        self._trial = _fused.bal_retract(K, T, p, xc, xp)
+        tl = _fused.bal_loss(*self._trial, self.pix, self.cidx, self.pidx, *self.robust)
+        sums = torch.cat([cur, tl, pred, pred.new_zeros(1)])
+        return self._result(sums, {"cur": 0, "loss": 1, "predicted": 2, "failed": 3})
+
+    def accept(self):
+        _copy_param(self.intr, self._trial[0])
+        _copy_param(self.poses, self._trial[1])
+        _copy_param(self.points, self._trial[2])
+
+    def device_step(self, strategy):
+        return None                 # every trial is driven from the host (LevenbergMarquardt._step_structured)
+
+
 def _input_key(input):
     items = input if isinstance(input, (tuple, list)) else (input,)
     return tuple((t.data_ptr(), tuple(t.shape), t.dtype, t._version) if torch.is_tensor(t) else id(t) for t in items)
@@ -685,6 +741,8 @@ def _recognize_by_signature(model, input, params, group, robust, solver, sparse,
     pass has the family's shape and the same sum of squares as the family's residual kernel on the same data
     (relative 1e-4).  Anything else falls through to the generic dense route."""
     from .solver import CG
+    if len(params) == 3:
+        return _recognize_bal(model, input, params, group, robust, solver, sparse, weight)
     if not isinstance(input, (tuple, list)) or len(params) not in (1, 2) or not _is_se3_param(params[0]):
         return None
     if params[0].dim() != 2 or params[0].dtype not in (torch.float32, torch.float64):
@@ -722,6 +780,54 @@ def _recognize_by_signature(model, input, params, group, robust, solver, sparse,
     return cand
 
 
+def _bal_residuals(input, K, T, P):
+    """Row-wise residuals of the BAL model (examples/module/ba `Reproj.project` - observations) with LieTensor ops."""
+    obs, ci, pi_ = input
+    ci = ci.long()
+    y = LieTensor(T.detach(), ltype=SE3_type)[ci].Act(P.detach()[pi_.long()])
+    n = -y[..., :2] / y[..., 2:]
+    rho = n.square().sum(-1, keepdim=True)
+    k = K.detach()[ci]
+    return k[..., :1] * (1 + k[..., 1:2] * rho + k[..., 2:3] * rho.square()) * n - obs
+
+
+def _bal_params_ok(K, T, P):
+    """(C,3) intrinsics, SE3 (C,7) poses and (P,3) points of one floating dtype on one CUDA device."""
+    return (_is_se3_param(T) and T.dim() == 2 and T.is_cuda and T.dtype in (torch.float32, torch.float64)
+            and all(torch.is_tensor(t) and not isinstance(t, LieTensor) and t.dim() == 2 and t.shape[1] == 3
+                    and t.dtype == T.dtype and t.device == T.device for t in (K, P))
+            and K.shape[0] == T.shape[0])
+
+
+def _recognize_bal(model, input, params, group, robust, solver, sparse, weight):
+    """A user module with three trainable parameters takes the BAL route when they are a plain (C,3), an SE3 (C,7) and a
+    plain (P,3), the input is (pixels (M,2), camera indices, point indices) in range, and its output equals the BAL
+    residual row by row (_same_residuals).  With P == C the shapes cannot tell intrinsics from points: both assignments
+    are tried."""
+    from .solver import CG
+    if not (isinstance(solver, CG) or sparse) or weight is not None or group is not None:
+        return None
+    if not isinstance(input, (tuple, list)) or len(input) != 3:
+        return None
+    obs, ci, pi_ = input
+    if not (torch.is_tensor(obs) and obs.dim() == 2 and obs.shape[1] == 2 and _is_index(ci, obs.shape[0])
+            and _is_index(pi_, obs.shape[0])):
+        return None
+    se3 = [p for p in params if _is_se3_param(p)]
+    if len(se3) != 1:
+        return None
+    T = se3[0]
+    K0, K1 = [p for p in params if p is not T]
+    for K, P in ((K0, K1), (K1, K0)):
+        if not (_bal_params_ok(K, T, P) and _in_range(ci, T.shape[0]) and _in_range(pi_, P.shape[0])):
+            continue
+        if _same_residuals(model, input, params, (obs.shape[0], 2), group, roles=(K, T, P)):
+            tol = solver.tol if isinstance(solver, CG) else 1e-8
+            maxiter = solver.maxiter if isinstance(solver, CG) else None
+            return BALProblem(model, obs, ci, pi_, _input_key(input), robust, tol, maxiter, (K, T, P))
+    return None
+
+
 def _family_residuals(input, params):
     """Row-wise residuals of the family the shapes point at, from the *original* (unsorted) inputs with ordinary
     LieTensor ops — an independent restatement used only to verify a user module at recognition time."""
@@ -738,9 +844,9 @@ def _family_residuals(input, params):
     return -y[..., :2] / y[..., 2:] - pixels
 
 
-def _same_residuals(model, input, params, shape, group, trials=2):
+def _same_residuals(model, input, params, shape, group, trials=2, roles=None):
     """A user module takes a fused family only if its output equals the family's residual ROW BY ROW (up to one global
-    sign) at the current parameters AND at randomly perturbed ones.  A single scalar at a single point is not
+    sign) at the current parameters AND at randomly perturbed ones (`roles` = (K, T, P): the BAL family).  A single scalar at a single point is not
     evidence: all-zero residuals at the start, a NaN loss, or a model that merely has the same norm there would pass
     it (ADVICE r1).  Non-finite outputs never match.  Parameters are restored exactly."""
     saved = [p.detach().clone() for p in params]
@@ -759,7 +865,7 @@ def _same_residuals(model, input, params, shape, group, trials=2):
                 if not torch.is_tensor(out) or isinstance(out, LieTensor) or tuple(out.shape) != tuple(shape):
                     ok = False
                     break
-                ref = _family_residuals(input, params)
+                ref = _family_residuals(input, params) if roles is None else _bal_residuals(input, *roles)
                 a, b = out.double(), ref.double()
                 scale = 1e-4 if out.dtype == torch.float32 else 1e-9
                 tol = scale * (1.0 + b.abs().max())
@@ -816,6 +922,19 @@ def recognize(model, input, params, group=None, robust=(0, 1.0), solver=None, sp
         tol = solver.tol if isinstance(solver, CG) else 1e-8
         maxiter = solver.maxiter if isinstance(solver, CG) else None
         return None if weight is not None else BAProblem(model, pix, cidx, pidx, _input_key(input), group, robust, tol, maxiter)
+    from ..module.ba import BALBundleAdjustment
+    if _is_builtin(model, BALBundleAdjustment):
+        K, T, P = model.intrinsics, model.poses, model.points_3d
+        ok = (len(params) == 3 and params[0] is K and params[1] is T and params[2] is P and _bal_params_ok(K, T, P)
+              and (isinstance(solver, CG) or sparse) and weight is None and group is None)
+        if not ok:
+            return None
+        pix, cidx, pidx = input
+        if not (_in_range(cidx, T.shape[0]) and _in_range(pidx, P.shape[0])):
+            raise IndexError("BALBundleAdjustment: camera / point index out of range")
+        tol = solver.tol if isinstance(solver, CG) else 1e-8
+        maxiter = solver.maxiter if isinstance(solver, CG) else None
+        return BALProblem(model, pix, cidx, pidx, _input_key(input), robust, tol, maxiter, (K, T, P))
     duck = _recognize_by_signature(model, input, params, group, robust, solver, sparse, weight)
     if duck is not None:
         return duck
