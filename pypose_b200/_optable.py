@@ -306,6 +306,55 @@ LM_OPS += [
      [("const REAL*", "Mn", "(2E,24)"), ("const int*", "nother", "(2E)"), ("const int*", "nptr", "(n+1)"), ("const REAL*", "x", "(n,6) step"),
       ("const REAL*", "g", "(n,6)"), ("double*", "ws", "ws[0] = x^T H x + 2 x^T g")],
      "TrustRegion 'predicted' reduction (J D)^T (2 R + J D), optim/strategy.py:143, by gather"),
+]
+
+
+# Sim3 pose graphs (csrc/sim3pgo.cu + the pcg2.cu kernels at block width 7): r = Log(Z^-1 A^-1 B) on Sim3 nodes, 7 unknowns
+# per node [tau phi sigma], J = sim3_Jl_inv(r) Adj(Z^-1 A^-1) with the reference's truncated series (operation.py:167-172).
+LM_OPS += [
+    ("b200_lm_sim3pgo_linearize",
+     [("const REAL*", "nodes", "(N,8) Sim3"), ("const REAL*", "Z", "(E,8) Sim3"), ("const int*", "ei", "(E)"), ("const int*", "ej", "(E)"),
+      ("const int*", "epos_i", "(E) slot of the edge in its first node's list"),
+      ("const int*", "epos_j", "(E) slot in its second node's list"),
+      ("REAL*", "Mn", "(2E,28) node-ordered blocks: upper triangle of J^T J, written at both slots"),
+      ("REAL*", "un", "(2E,7) -J^T r at the first node's slot, +J^T r at the second's"),
+      ("double*", "ws", "ws[0] = sum rho(|r|^2)"), ("int", "robust", ""), ("double", "delta", "")],
+     "modjac + J^T J of optimizer.py:645-656 for the Sim3 pose graph (examples/module/pgo/pgo.py:15-25 on Sim3 nodes), "
+     "written in node order (no atomics downstream)"),
+    ("b200_lm_sim3pgo_loss",
+     [("const REAL*", "nodes", "(N,8)"), ("const REAL*", "Z", "(E,8)"), ("const int*", "ei", "(E)"), ("const int*", "ej", "(E)"),
+      ("double*", "ws", "ws[0] = sum rho(|r|^2)"), ("int", "robust", ""), ("double", "delta", "")],
+     "RobustModel.loss of the Sim3 pose graph, optimizer.py:118-125"),
+    ("b200_lm_sim3pgo_node_sums",
+     [("const REAL*", "Mn", "(2E,28)"), ("const REAL*", "un", "(2E,7)"), ("const int*", "nptr", "(N+1) offsets per node"),
+      ("REAL*", "Hd", "(N,28) diagonal blocks of J^T J"), ("REAL*", "g", "(N,7) J^T R")],
+     "b200_lm_pgo2_node_sums at block width 7"),
+    ("b200_lm_sim3pgo_damp_inv",
+     [("const REAL*", "H", "(n,28) packed 7x7 blocks"), ("double", "scale", "prod(1+damping) over trials"),
+      ("double", "dmin", "diag clamp min"), ("double", "dmax", "diag clamp max"), ("REAL*", "Hd", "(n,28) damped blocks or NULL"),
+      ("REAL*", "extra", "(n,7) amount added to the diagonal, or NULL"),
+      ("REAL*", "Minv", "(n,28) inverses of the damped blocks or NULL")],
+     "clamp + cumulative damping of the diagonal (optimizer.py:657/666) on 7x7 Sim3 node blocks"),
+    ("b200_lm_sim3pgo_pcg",
+     [("const REAL*", "Mn", "(2E,28) node-ordered blocks"), ("const int*", "nother", "(2E) opposite node of each slot"),
+      ("const int*", "nptr", "(n+1)"), ("const REAL*", "Minv", "(n,28) block-Jacobi preconditioner"),
+      ("const REAL*", "extra", "(n,7) clamp / damping added to diag H"), ("const REAL*", "g", "(n,7); solves (H+extra) x = -g"),
+      ("REAL*", "x", "(n,7)"), ("REAL*", "r", "(n,7)"), ("REAL*", "z", "(n,7)"), ("REAL*", "p0", "(n,7) direction, even iterations"),
+      ("REAL*", "p1", "(n,7) direction, odd iterations"), ("REAL*", "q", "(n,7)"), ("REAL*", "xbest", "(n,7)"),
+      ("double*", "cg", "(16) state, see b200_lm_pgo_pcg"), ("double*", "ws", ""), ("double", "tol", ""),
+      ("long long", "maxiter", ""), ("long long", "first_iter", ""), ("long long", "iters", "")],
+     "b200_lm_pgo2_pcg at block width 7: PCG.forward loop, optim/solver.py:312-340, no atomics, bit-reproducible"),
+    ("b200_lm_sim3pgo_cg_finish",
+     [("REAL*", "x", "(n,7)"), ("const REAL*", "xbest", "(n,7)"), ("const double*", "cg", "(16) state")],
+     "x <- best iterate unless the PCG converged (the best-iterate guard of b200_lm_cg_finish at width 7)"),
+    ("b200_lm_sim3pgo_predicted",
+     [("const REAL*", "Mn", "(2E,28)"), ("const int*", "nother", "(2E)"), ("const int*", "nptr", "(n+1)"), ("const REAL*", "x", "(n,7) step"),
+      ("const REAL*", "g", "(n,7)"), ("double*", "ws", "ws[0] = x^T H x + 2 x^T g")],
+     "TrustRegion 'predicted' reduction of the Sim3 pose graph, optim/strategy.py:143, by gather"),
+]
+
+
+LM_OPS += [
     ("b200_lm_reproj2_accum",
      [("const REAL*", "nodes", "(N,7) SE3 poses"), ("const REAL*", "pts", "(m,3) points in the frame of pose a, rows sorted by pair"),
       ("const REAL*", "pix", "(m,2)"), ("const int*", "pseg", "(E+1) row offsets per ordered pose pair"),

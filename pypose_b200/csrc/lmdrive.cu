@@ -67,6 +67,22 @@ template <typename CT> struct Api;
   };
 B200_API(f32, float)
 B200_API(f64, double)
+// family 2 (Sim3 pose graph): the same sequence at block width 7 (entry points of the same signatures)
+template <typename CT> struct Sim3Api;
+#define B200_SIM3_API(SFX, CT)                                                                                        \
+  template <> struct Sim3Api<CT> {                                                                                    \
+    static constexpr auto linearize = b200_lm_sim3pgo_linearize_##SFX;                                                \
+    static constexpr auto node_sums = b200_lm_sim3pgo_node_sums_##SFX;                                                \
+    static constexpr auto damp_inv = b200_lm_sim3pgo_damp_inv_##SFX;                                                  \
+    static constexpr auto pcg = b200_lm_sim3pgo_pcg_##SFX;                                                            \
+    static constexpr auto finish = b200_lm_sim3pgo_cg_finish_##SFX;                                                   \
+    static constexpr auto predicted = b200_lm_sim3pgo_predicted_##SFX;                                                \
+    static constexpr auto exp = b200_sim3_exp_fwd_##SFX;                                                              \
+    static constexpr auto mul = b200_Sim3_mul_fwd_##SFX;                                                              \
+    static constexpr auto loss = b200_lm_sim3pgo_loss_##SFX;                                                          \
+  };
+B200_SIM3_API(f32, float)
+B200_SIM3_API(f64, double)
 
 static LmCtl ctl_from(const double* c) {
   LmCtl k;
@@ -78,8 +94,11 @@ static LmCtl ctl_from(const double* c) {
 
 template <typename CT> static int pgo_step(b200_pgo_step_args* a, void* stream) {
   using A = Api<CT>;
+  using S = Sim3Api<CT>;
   cudaStream_t s = (cudaStream_t)stream;
   const long long N = a->N, E = a->E;
+  const bool sim3 = a->family == 2;
+  const long long W = sim3 ? 7 : 6, D = sim3 ? 8 : 7;      // unknowns per node, parameter width
   CT* nodes = (CT*)a->nodes;
   CT *Mn = (CT*)a->Mn, *un = (CT*)a->un, *Hd = (CT*)a->Hd, *g = (CT*)a->g, *extra = (CT*)a->extra, *Minv = (CT*)a->Minv;
   CT *x = (CT*)a->x, *r = (CT*)a->r, *z = (CT*)a->z, *p0 = (CT*)a->p0, *p1 = (CT*)a->p1, *q = (CT*)a->q, *xbest = (CT*)a->xbest;
@@ -88,22 +107,25 @@ template <typename CT> static int pgo_step(b200_pgo_step_args* a, void* stream) 
   if (!a->retry) {                                       // linearise at the current parameters (kept across rejected trials)
     if (a->family == 0)
       B200_TRY(A::linearize(nodes, (const CT*)a->Z, a->ei, a->ej, a->epos_i, a->epos_j, Mn, un, a->ws3, a->robust, a->delta, E, stream));
+    else if (sim3)
+      B200_TRY(S::linearize(nodes, (const CT*)a->Z, a->ei, a->ej, a->epos_i, a->epos_j, Mn, un, a->ws3, a->robust, a->delta, E, stream));
     else
       B200_TRY(A::accum2(nodes, (const CT*)a->pts, (const CT*)a->pix, a->pseg, a->pa, a->pb, a->intr, a->epos_i, a->epos_j, Mn, un,
                          a->ws3, a->robust, a->delta, E, stream));
-    B200_TRY(A::node_sums(Mn, un, a->nptr, Hd, g, N, stream));
+    B200_TRY((sim3 ? S::node_sums : A::node_sums)(Mn, un, a->nptr, Hd, g, N, stream));
   }
-  B200_TRY(A::damp_inv(Hd, a->scale, a->dmin, a->dmax, (CT*)nullptr, extra, Minv, N, stream));
+  B200_TRY((sim3 ? S::damp_inv : A::damp_inv)(Hd, a->scale, a->dmin, a->dmax, (CT*)nullptr, extra, Minv, N, stream));
   // PCG: chunks of iterations without host involvement; after each chunk a one-thread kernel publishes the CG state
-  const long long maxiter = a->maxiter > 0 ? a->maxiter : 10 * 6 * N;
+  const long long maxiter = a->maxiter > 0 ? a->maxiter : 10 * W * N;
+  const auto pcg = sim3 ? S::pcg : A::pcg;
   long long it = 0;
   double cgseq = host[32];
   for (;;) {
     long long n = (it == 0 && a->hint > 0) ? a->hint : 8;
     if (n > maxiter - it) n = maxiter - it;
     if (n < 1) n = 1;
-    B200_TRY(A::pcg(Mn, a->nother, a->nptr, Minv, extra, g, x, r, z, p0, p1, q, xbest, a->cg, a->ws0, a->tol, maxiter, it, n, N,
-                    stream));
+    B200_TRY(pcg(Mn, a->nother, a->nptr, Minv, extra, g, x, r, z, p0, p1, q, xbest, a->cg, a->ws0, a->tol, maxiter, it, n, N,
+                 stream));
     it += n;
     cgseq += 1.0;
     publish_kernel<<<1, 32, 0, s>>>(a->cg, 16, a->host + 16, cgseq);
@@ -112,15 +134,16 @@ template <typename CT> static int pgo_step(b200_pgo_step_args* a, void* stream) 
     if (host[16 + 5] != 0.0 || it >= maxiter) break;      // done flag of the CG state
   }
   a->iters_out = (long long)host[16 + 6];
-  B200_TRY(A::finish(x, xbest, a->cg, N, stream));
-  B200_TRY(A::predicted(Mn, a->nother, a->nptr, x, g, a->ws2, N, stream));
-  B200_TRY(A::exp(x, X7, N, stream));                    // retraction P' = Exp(D) P  (lietensor.py:442-444)
-  B200_TRY(A::mul(X7, nodes, Pt, N, stream));
+  B200_TRY((sim3 ? S::finish : A::finish)(x, xbest, a->cg, N, stream));
+  B200_TRY((sim3 ? S::predicted : A::predicted)(Mn, a->nother, a->nptr, x, g, a->ws2, N, stream));
+  B200_TRY((sim3 ? S::exp : A::exp)(x, X7, N, stream));  // retraction P' = Exp(D) P  (lietensor.py:442-444)
+  B200_TRY((sim3 ? S::mul : A::mul)(X7, nodes, Pt, N, stream));
   if (a->family == 0) B200_TRY(A::loss0(Pt, (const CT*)a->Z, a->ei, a->ej, a->ws1, a->robust, a->delta, E, stream));
+  else if (sim3) B200_TRY(S::loss(Pt, (const CT*)a->Z, a->ei, a->ej, a->ws1, a->robust, a->delta, E, stream));
   else B200_TRY(A::loss1(Pt, (const CT*)a->pts, (const CT*)a->pix, a->pseg, a->pa, a->pb, a->intr, a->ws1, a->robust, a->delta, E, stream));
   host[ST_SIZE - 1] = -1.0;
   pgo_decide_kernel<<<1, 32, 0, s>>>(a->ws3, a->ws1, a->ws2, ctl_from(a->ctl), a->st, a->host, (double)a->seq);
-  commit_kernel<CT><<<lm_grid(N * 7, kLmThreads), kLmThreads, 0, s>>>(a->st, Pt, nodes, N * 7);
+  commit_kernel<CT><<<lm_grid(N * D, kLmThreads), kLmThreads, 0, s>>>(a->st, Pt, nodes, N * D);
   B200_TRY((int)cudaGetLastError());
   return spin_until(host + (ST_SIZE - 1), (double)a->seq, s);
 }

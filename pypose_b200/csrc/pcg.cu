@@ -18,23 +18,32 @@ namespace b200pose {
 
 
 // diag <- clamp(diag, dmin, dmax) * scale (optimizer.py:657 + cumulative :666); optional outputs: the damped block,
-// the amount added to the diagonal, the inverse of the damped block.
-template <typename T>
-__global__ void __launch_bounds__(kLmThreads) blk6_damp_inv_kernel(const T* __restrict__ H, T scale, T dmin, T dmax,
+// the amount added to the diagonal, the inverse of the damped block.  W = 6: SE3 blocks; W = 7: Sim3 pose-graph blocks.
+template <int W, typename T> __device__ __forceinline__ void blkw_unpack(const T* a, T (&A)[W][W]) {
+  if constexpr (W == 6) sym6_unpack(a, A);
+  else symn_unpack<T, W>(a, A);
+}
+template <int W, typename T> __device__ __forceinline__ void blkw_pack(const T (&A)[W][W], T* a) {
+  if constexpr (W == 6) sym6_pack(A, a);
+  else symn_pack<T, W>(A, a);
+}
+template <typename T, int W>
+__global__ void __launch_bounds__(kLmThreads) blkw_damp_inv_kernel(const T* __restrict__ H, T scale, T dmin, T dmax,
                                                                     T* __restrict__ Hd, T* __restrict__ extra,
                                                                     T* __restrict__ Minv, long long n) {
+  constexpr int NP = packed_words<W>();
   for (long long i = (long long)blockIdx.x * kLmThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kLmThreads) {
-    T A[6][6], Ai[6][6];
-    sym6_unpack(H + i * 21, A);
+    T A[W][W], Ai[W][W];
+    blkw_unpack<W>(H + i * NP, A);
 #pragma unroll
-    for (int k = 0; k < 6; ++k) {
+    for (int k = 0; k < W; ++k) {
       const T d = A[k][k];
       const T c = (d < dmin ? dmin : (d > dmax ? dmax : d)) * scale;
-      if (extra) extra[i * 6 + k] = c - d;
+      if (extra) extra[i * W + k] = c - d;
       A[k][k] = c;
     }
-    if (Hd) sym6_pack(A, Hd + i * 21);
-    if (Minv) { spd_inverse<T, 6>(A, Ai); sym6_pack(Ai, Minv + i * 21); }
+    if (Hd) blkw_pack<W>(A, Hd + i * NP);
+    if (Minv) { spd_inverse<T, W>(A, Ai); blkw_pack<W>(Ai, Minv + i * NP); }
   }
 }
 
@@ -172,25 +181,26 @@ __global__ void __launch_bounds__(kLmThreads) pgo_predicted_edge_kernel(const T*
 }
 
 // used by pcg2.cu (node-ordered two-kernel iteration): x = 0, r = -b, z = M^-1 r (stored through the `p` slot), state reset
-template <typename T>
+template <typename T, int W>
 void pcg_launch_init(const T* Minv, const T* b, T* x, T* r, T* z, T* q, double* cg, double* ws, double tol, double maxiter,
                      long long n, cudaStream_t st) {
-  cg_init_kernel<T><<<lm_grid(n, kLmThreads), kLmThreads, 0, st>>>(Minv, b, (T)-1, (const T*)nullptr, 0, x, r, z, q, cg, ws, tol,
-                                                                  maxiter, n);
+  cg_init_kernel<T, W><<<lm_grid(n, kLmThreads), kLmThreads, 0, st>>>(Minv, b, (T)-1, (const T*)nullptr, 0, x, r, z, q, cg, ws,
+                                                                     tol, maxiter, n);
 }
-template <typename T>
+template <typename T, int W>
 void pcg_launch_update(const T* Minv, const T* p, const T* q, T* x, T* r, T* z, T* xbest, double* cg, double* ws, int par,
                        long long n, cudaStream_t st) {
-  cg_update_kernel<T><<<lm_grid(n, kLmThreads), kLmThreads, 0, st>>>(Minv, p, q, x, r, z, xbest, cg, ws, par, n);
+  cg_update_kernel<T, W><<<lm_grid(n, kLmThreads), kLmThreads, 0, st>>>(Minv, p, q, x, r, z, xbest, cg, ws, par, n);
 }
-template void pcg_launch_init<float>(const float*, const float*, float*, float*, float*, float*, double*, double*, double, double,
-                                     long long, cudaStream_t);
-template void pcg_launch_init<double>(const double*, const double*, double*, double*, double*, double*, double*, double*, double,
-                                      double, long long, cudaStream_t);
-template void pcg_launch_update<float>(const float*, const float*, const float*, float*, float*, float*, float*, double*, double*,
-                                       int, long long, cudaStream_t);
-template void pcg_launch_update<double>(const double*, const double*, const double*, double*, double*, double*, double*, double*,
-                                        double*, int, long long, cudaStream_t);
+#define PCG_LAUNCH_INST(T, W)                                                                                        \
+  template void pcg_launch_init<T, W>(const T*, const T*, T*, T*, T*, T*, double*, double*, double, double, long long,     \
+                                      cudaStream_t);                                                                  \
+  template void pcg_launch_update<T, W>(const T*, const T*, const T*, T*, T*, T*, T*, double*, double*, int, long long,   \
+                                        cudaStream_t);
+PCG_LAUNCH_INST(float, 6)
+PCG_LAUNCH_INST(double, 6)
+PCG_LAUNCH_INST(float, 7)
+PCG_LAUNCH_INST(double, 7)
 
 }  // namespace b200pose
 
@@ -283,7 +293,19 @@ static int ba_pcg_run(const CT* Y4, const CT* poses, const int* pidx, const int*
   B200_EXPORT int b200_lm_blk6_damp_inv_##SFX(const CT* H, double scale, double dmin, double dmax, CT* Hd, CT* extra, \
                                               CT* Minv, long long n, void* stream) {                                  \
     if (n <= 0) return 0;                                                                                             \
-    LM_LAUNCH(blk6_damp_inv_kernel<CT>, n, stream, H, (CT)scale, (CT)dmin, (CT)dmax, Hd, extra, Minv, n);             \
+    LM_LAUNCH((blkw_damp_inv_kernel<CT, 6>), n, stream, H, (CT)scale, (CT)dmin, (CT)dmax, Hd, extra, Minv, n);        \
+    return (int)cudaGetLastError();                                                                                   \
+  }                                                                                                                   \
+  B200_EXPORT int b200_lm_sim3pgo_damp_inv_##SFX(const CT* H, double scale, double dmin, double dmax, CT* Hd,         \
+                                                 CT* extra, CT* Minv, long long n, void* stream) {                    \
+    if (n <= 0) return 0;                                                                                             \
+    LM_LAUNCH((blkw_damp_inv_kernel<CT, 7>), n, stream, H, (CT)scale, (CT)dmin, (CT)dmax, Hd, extra, Minv, n);        \
+    return (int)cudaGetLastError();                                                                                   \
+  }                                                                                                                   \
+  B200_EXPORT int b200_lm_sim3pgo_cg_finish_##SFX(CT* x, const CT* xbest, const double* cg, long long n,              \
+                                                  void* stream) {                                                     \
+    if (n <= 0) return 0;                                                                                             \
+    LM_LAUNCH(cg_finish_kernel<CT>, n * 7, stream, x, xbest, cg, n * 7);                                              \
     return (int)cudaGetLastError();                                                                                   \
   }                                                                                                                   \
   B200_EXPORT int b200_lm_pt3_damp_inv_##SFX(const CT* H, double scale, double dmin, double dmax, CT* Hinv,           \

@@ -324,43 +324,67 @@ def _run_chunks(enqueue, cg, maxiter, hint=0):
 
 
 def pgo_linearize_nodes(kind, prob, nodes, robust, delta):
-    """Blocks of the current linearisation directly in node order (csrc/lm.cu store_edge_blocks) and, by gather, the
-    diagonal blocks Hd and J^T R.  kind: "pgo" (Log(Z^-1 A^-1 B) edges) or "reproj2" (pose pairs)."""
+    """Blocks of the current linearisation directly in node order (csrc/lm.cu store_edge_blocks, csrc/sim3pgo.cu) and, by
+    gather, the diagonal blocks Hd and J^T R.  kind: "pgo" (Log(Z^-1 A^-1 B) edges), "reproj2" (pose pairs) or "sim3"
+    (Log(Z^-1 A^-1 B) on Sim3 nodes: 7 unknowns per node, 28-word slots)."""
     E, N = prob.ei.shape[0], prob.nptr.shape[0] - 1
     E2 = 2 * E
     dt, dev = nodes.dtype, nodes.device
     ws = _workspace(dev)
-    Mn, un = torch.empty(E2, 24, dtype=dt, device=dev), torch.empty(E2, 6, dtype=dt, device=dev)
+    W, slot, pw = (7, 28, 28) if kind == "sim3" else (6, 24, 21)
+    Mn, un = torch.empty(E2, slot, dtype=dt, device=dev), torch.empty(E2, W, dtype=dt, device=dev)
     if kind == "pgo":
         _launch("b200_lm_pgo_linearize_n", nodes, [_p(nodes), _p(prob.Z), _p(prob.ei), _p(prob.ej), _p(prob.epos_i), _p(prob.epos_j),
                                                    _p(Mn), _p(un), _p(ws), int(robust), float(delta)], E)
+    elif kind == "sim3":
+        _launch("b200_lm_sim3pgo_linearize", nodes, [_p(nodes), _p(prob.Z), _p(prob.ei), _p(prob.ej), _p(prob.epos_i),
+                                                     _p(prob.epos_j), _p(Mn), _p(un), _p(ws), int(robust), float(delta)], E)
     else:
         k = (ctypes.c_double * 5)(*prob.intr)
         _launch("b200_lm_reproj2_accum_n", nodes, [_p(nodes), _p(prob.pts), _p(prob.pix), _p(prob.pseg), _p(prob.pa), _p(prob.pb),
                                                    ctypes.addressof(k), _p(prob.epos_i), _p(prob.epos_j), _p(Mn), _p(un), _p(ws),
                                                    int(robust), float(delta)], E)
     cur = ws[:1].clone()
-    Hd, g = torch.empty(N, 21, dtype=dt, device=dev), torch.empty(N, 6, dtype=dt, device=dev)
-    _launch("b200_lm_pgo2_node_sums", nodes, [_p(Mn), _p(un), _p(prob.nptr), _p(Hd), _p(g)], N)
+    Hd, g = torch.empty(N, pw, dtype=dt, device=dev), torch.empty(N, W, dtype=dt, device=dev)
+    if kind == "sim3":
+        _launch("b200_lm_sim3pgo_node_sums", nodes, [_p(Mn), _p(un), _p(prob.nptr), _p(Hd), _p(g)], N)
+    else:
+        _launch("b200_lm_pgo2_node_sums", nodes, [_p(Mn), _p(un), _p(prob.nptr), _p(Hd), _p(g)], N)
     return Mn, Hd, g, cur
 
 
 def pgo_solve_nodes(Mn, nother, nptr, Hd, g, scale, dmin, dmax, tol, maxiter, hint=0):
     """(H + clamp/damping) x = -g on node-ordered blocks (csrc/pcg2.cu): two launches per iteration, no atomics.
-    Returns x (n,6), iterations, predicted (1,) fp64 on device."""
-    dev, dt, n = Mn.device, Mn.dtype, Hd.shape[0]
+    The block width W (6: SE3 nodes, 7: Sim3 nodes) is g's.  Returns x (n,W), iterations, predicted (1,) fp64 on device."""
+    dev, dt, n, W = Mn.device, Mn.dtype, Hd.shape[0], g.shape[1]
     ws, cg = _workspace(dev), _cg(dev)
-    extra = torch.empty(n, 6, dtype=dt, device=dev)
-    Minv = torch.empty(n, 21, dtype=dt, device=dev)
+    extra = torch.empty(n, W, dtype=dt, device=dev)
+    Minv = torch.empty_like(Hd)
+    x, r, z, p0, p1, q, xbest = (torch.empty(n, W, dtype=dt, device=dev) for _ in range(7))
+    maxiter = int(maxiter) if maxiter is not None else 10 * W * n
+    if W == 7:
+        _launch("b200_lm_sim3pgo_damp_inv", Mn, [_p(Hd), float(scale), float(dmin), float(dmax), _p(None), _p(extra), _p(Minv)], n)
+        iters = _run_chunks(lambda it0, k: _launch("b200_lm_sim3pgo_pcg", Mn, [
+            _p(Mn), _p(nother), _p(nptr), _p(Minv), _p(extra), _p(g), _p(x), _p(r), _p(z), _p(p0), _p(p1), _p(q), _p(xbest),
+            _p(cg), _p(ws), float(tol), maxiter, it0, k], n), cg, maxiter, hint)
+        _launch("b200_lm_sim3pgo_cg_finish", Mn, [_p(x), _p(xbest), _p(cg)], n)
+        _launch("b200_lm_sim3pgo_predicted", Mn, [_p(Mn), _p(nother), _p(nptr), _p(x), _p(g), _p(ws)], n)
+        return x, iters, ws[:1].clone()
     _launch("b200_lm_blk6_damp_inv", Mn, [_p(Hd), float(scale), float(dmin), float(dmax), _p(None), _p(extra), _p(Minv)], n)
-    x, r, z, p0, p1, q, xbest = (torch.empty(n, 6, dtype=dt, device=dev) for _ in range(7))
-    maxiter = int(maxiter) if maxiter is not None else 10 * 6 * n
     iters = _run_chunks(lambda it0, k: _launch("b200_lm_pgo2_pcg", Mn, [
         _p(Mn), _p(nother), _p(nptr), _p(Minv), _p(extra), _p(g), _p(x), _p(r), _p(z), _p(p0), _p(p1), _p(q), _p(xbest),
         _p(cg), _p(ws), float(tol), maxiter, it0, k], n), cg, maxiter, hint)
     _launch("b200_lm_cg_finish", Mn, [_p(x), _p(xbest), _p(cg)], n)
     _launch("b200_lm_pgo2_predicted", Mn, [_p(Mn), _p(nother), _p(nptr), _p(x), _p(g), _p(ws)], n)
     return x, iters, ws[:1].clone()
+
+
+def sim3pgo_loss(nodes, Z, ei, ej, robust=0, delta=1.0):
+    """(1,) fp64 device tensor: sum rho(|r|^2) of the Sim3 pose graph at the given (N,8) nodes."""
+    nodes, Z = _same(nodes, Z)
+    ws = _workspace(nodes.device)
+    _launch("b200_lm_sim3pgo_loss", nodes, [_p(nodes), _p(Z), _p(ei), _p(ej), _p(ws), int(robust), float(delta)], Z.shape[0])
+    return ws[:1].clone()
 
 
 _NOCOMM = [None, 0, 1, 0, 0, 0, None]

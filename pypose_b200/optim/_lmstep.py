@@ -182,10 +182,13 @@ class PgoDeviceStep:
         N, E = nodes.shape[0], prob.ei.shape[0]
         self.device, self.dtype, self.comm = dev, dt, None
         new = lambda *shape: torch.empty(*shape, dtype=dt, device=dev)
-        self.buf = {"Mn": new(2 * E, 24), "un": new(2 * E, 6), "Hd": new(N, 21), "g": new(N, 6), "extra": new(N, 6),
-                    "Minv": new(N, 21), "x": new(N, 6), "r": new(N, 6), "z": new(N, 6), "p0": torch.zeros(N, 6, dtype=dt, device=dev),
-                    "p1": torch.zeros(N, 6, dtype=dt, device=dev), "q": new(N, 6), "xbest": new(N, 6), "X7": new(N, 7),
-                    "Pt": new(N, 7)}
+        family = {"pgo": 0, "reproj2": 1, "sim3": 2}[prob.kind]
+        # block width W, slot words, packed block words and parameter width D of the family (include/b200pose.h)
+        W, slot, pw, D = (7, 28, 28, 8) if family == 2 else (6, 24, 21, 7)
+        self.buf = {"Mn": new(2 * E, slot), "un": new(2 * E, W), "Hd": new(N, pw), "g": new(N, W), "extra": new(N, W),
+                    "Minv": new(N, pw), "x": new(N, W), "r": new(N, W), "z": new(N, W), "p0": torch.zeros(N, W, dtype=dt, device=dev),
+                    "p1": torch.zeros(N, W, dtype=dt, device=dev), "q": new(N, W), "xbest": new(N, W), "X7": new(N, D),
+                    "Pt": new(N, D)}
         n = _C.lib().b200_lm_workspace_doubles
         n.restype = ctypes.c_longlong
         self.W = torch.zeros(4, int(n()), dtype=torch.float64, device=dev)        # this problem's own reduction slots
@@ -193,7 +196,7 @@ class PgoDeviceStep:
         self.host = torch.zeros(40, dtype=torch.float64).pin_memory()
         self.state = None
         a = self.args = PgoStepArgs()
-        a.family, a.is64 = (0 if prob.kind == "pgo" else 1), int(dt == torch.float64)
+        a.family, a.is64 = family, int(dt == torch.float64)
         a.N, a.E = N, E
         a.Z = prob.Z.data_ptr() if prob.Z is not None else None
         if prob.kind == "reproj2":

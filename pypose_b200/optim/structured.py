@@ -19,7 +19,7 @@ import torch
 
 from .. import _C
 from ..lietensor import lietensor as _lt
-from ..lietensor.lietensor import LieTensor, Parameter, SE3_type
+from ..lietensor.lietensor import LieTensor, Parameter, SE3_type, Sim3_type
 from ..lietensor.scan import _sms
 from . import _fused  # noqa: F401  (registers the ops)
 from . import _lmstep
@@ -46,6 +46,12 @@ def _retract_se3(D, poses):
         X = _C.launch_rows("b200_se3_exp_fwd", [D.contiguous()], [7])[0]
         return _C.launch_rows("b200_SE3_mul_fwd", [X, poses.contiguous()], [7])[0]
     return (LieTensor(D, ltype=_lt.se3_type).Exp() * LieTensor(poses, ltype=SE3_type)).tensor()
+
+
+def _retract_sim3(D, nodes):
+    """Exp(D) * nodes for (n,7) steps and (n,8) Sim3 rows (CUDA only: the Sim3 pose-graph route runs on one GPU)."""
+    X = _C.launch_rows("b200_sim3_exp_fwd", [D.contiguous()], [8])[0]
+    return _C.launch_rows("b200_Sim3_mul_fwd", [X, nodes.contiguous()], [8])[0]
 
 
 class _Problem:
@@ -284,6 +290,7 @@ class PGOProblem(_Problem):
     per-edge scatter route (information matrices, or edges sharded over a process group): per-edge M_e = J^T J and
                u_e = J^T r (one kernel), diagonal blocks + gradient by atomics, a matvec that walks the edges
                (csrc/lm.cu lm_pgo_spmv_kernel).  With a group, Hd, g, every matvec and the scalars are all-reduced."""
+    D = 7                       # parameter width of a node (Sim3PGOProblem: 8)
 
     def __init__(self, model, edges, Z, key, group, robust, tol, maxiter, param=None, weight=None):
         self.model, self.key, self.group, self.robust = model, key, group, robust
@@ -292,7 +299,7 @@ class PGOProblem(_Problem):
         self.dtype = self.param.dtype
         self.ei = edges[..., 0].to(torch.int32).contiguous()
         self.ej = edges[..., 1].to(torch.int32).contiguous()
-        self.Z = None if Z is None else Z.tensor().to(self.dtype).reshape(-1, 7).contiguous()
+        self.Z = None if Z is None else Z.tensor().to(self.dtype).reshape(-1, self.D).contiguous()
         # information matrices (examples/module/pgo/pgo.py:75 `weight=infos`): (E,6,6) or one (6,6) for all edges
         self.W = None if weight is None else weight.to(self.dtype).reshape(-1, 36).contiguous()
         self.kind = "pgo"
@@ -301,7 +308,7 @@ class PGOProblem(_Problem):
         keys = torch.cat([self.ei, self.ej]).long()
         order = torch.sort(keys, stable=True)[1]
         self.nother = torch.cat([self.ej, self.ei])[order].contiguous()
-        N = self.param.tensor().reshape(-1, 7).shape[0]
+        N = self.param.tensor().reshape(-1, self.D).shape[0]
         self.nptr = torch.zeros(N + 1, dtype=torch.int32, device=keys.device)
         self.nptr[1:] = torch.cumsum(torch.bincount(keys, minlength=N), 0).to(torch.int32)
         pos = torch.empty(2 * E, dtype=torch.int32, device=keys.device)
@@ -316,7 +323,7 @@ class PGOProblem(_Problem):
                 and self.weight_key == (None if weight is None else _input_key(weight)))
 
     def _nodes(self):
-        return self.param.tensor().reshape(-1, 7)
+        return self.param.tensor().reshape(-1, self.D)
 
     # the two family-specific pieces (overridden by Reproj2Problem): per-edge blocks and the loss at given nodes
     def _loss_at(self, nodes):
@@ -392,8 +399,11 @@ class PGOProblem(_Problem):
             predicted = _allreduce(predicted, self.group)
         return self._finish_trial(D, predicted, cur)
 
+    def _retract(self, D, nodes):
+        return _retract_se3(D, nodes)
+
     def _finish_trial(self, D, predicted, cur):
-        self._trial = _retract_se3(D, self._nodes())
+        self._trial = self._retract(D, self._nodes())
         tl = self._loss_at(self._trial)
         shard = _allreduce(torch.cat([cur, tl]), self.group)
         return self._result(torch.cat([shard, predicted, predicted.new_zeros(1)]),
@@ -455,6 +465,29 @@ class Reproj2Problem(PGOProblem):
         M, u, cur = _fused.call("lm_reproj2_accum", nodes, self.pts, self.pix, self.pseg, self.pa, self.pb, self.intr,
                                 *self.robust)
         return M, u, cur, None
+
+
+class Sim3PGOProblem(PGOProblem):
+    """Sim3 pose graph r_e = Log(Z_e^-1 A^-1 B) on Sim3 nodes (examples/module/pgo `PoseGraph` with pp.Sim3 nodes, as in
+    monocular loop closure, where scale drifts).  A node has 7 unknowns [tau phi sigma]; J = sim3_Jl_inv(r) Adj(Z^-1 A^-1)
+    with the reference's truncated series (csrc/sim3pgo_math.cuh).  The blocks are written in node order and solved by the
+    PCG of csrc/pcg2.cu at block width 7; the update is Exp(D) P.  One CUDA device, no process group, no information
+    matrices (those graphs keep the generic route)."""
+    D = 8
+
+    def __init__(self, model, edges, Z, key, robust, tol, maxiter, param=None):
+        super().__init__(model, edges, Z, key, None, robust, tol, maxiter, param=param)
+        self.kind = "sim3"
+
+    def _loss_at(self, nodes):
+        return _fused.sim3pgo_loss(nodes, self.Z, self.ei, self.ej, *self.robust)
+
+    def linearize(self):
+        Mn, Hd, g, cur = _fused.pgo_linearize_nodes(self.kind, self, self._nodes(), *self.robust)
+        return (Mn,), Hd, g, cur, None
+
+    def _retract(self, D, nodes):
+        return _retract_sim3(D, nodes)
 
 
 def _peer_allreduce(prob, param, max_elems):
@@ -799,6 +832,37 @@ def _bal_params_ok(K, T, P):
             and K.shape[0] == T.shape[0])
 
 
+def _recognize_sim3(model, input, params, group, robust, solver, sparse, weight):
+    """A Sim3 pose graph takes the Sim3 route when an iterative solve was asked for (solver=PCG()/CG() or sparse=True), the
+    one trainable parameter is an (N,8) Sim3 Parameter on a CUDA device, the input is (edges (E,2) in range, Sim3 Z (E,8)) of
+    the parameter's dtype and device, there are no information matrices and no process group, and the model is the
+    built-in PoseGraph or its output equals the Sim3 pose-graph residual row by row (_same_residuals)."""
+    from .solver import CG
+    from ..module.pgo import PoseGraph
+    P = params[0]
+    if not (isinstance(solver, CG) or sparse) or weight is not None or group is not None:
+        return None
+    if not (isinstance(P, Parameter) and P.is_cuda and P.dim() == 2 and P.dtype in (torch.float32, torch.float64)):
+        return None
+    if not isinstance(input, (tuple, list)) or len(input) != 2:
+        return None
+    edges, Z = input
+    if not (torch.is_tensor(edges) and edges.dtype in (torch.int64, torch.int32) and edges.dim() == 2 and edges.shape[1] == 2
+            and edges.device == P.device and isinstance(Z, LieTensor) and Z.ltype is Sim3_type
+            and Z.shape == (edges.shape[0], 8) and Z.dtype == P.dtype and Z.device == P.device):
+        return None
+    tol = solver.tol if isinstance(solver, CG) else 1e-8
+    maxiter = solver.maxiter if isinstance(solver, CG) else None
+    if _is_builtin(model, PoseGraph):
+        if P is not model.nodes:
+            return None
+        if not _in_range(edges, P.shape[0]):
+            raise IndexError("PoseGraph: edge index out of range")
+    elif not (_in_range(edges, P.shape[0]) and _same_residuals(model, input, params, (edges.shape[0], 7), group)):
+        return None
+    return Sim3PGOProblem(model, edges, Z, _input_key(input), robust, tol, maxiter, param=P)
+
+
 def _recognize_bal(model, input, params, group, robust, solver, sparse, weight):
     """A user module with three trainable parameters takes the BAL route when they are a plain (C,3), an SE3 (C,7) and a
     plain (P,3), the input is (pixels (M,2), camera indices, point indices) in range, and its output equals the BAL
@@ -831,7 +895,7 @@ def _recognize_bal(model, input, params, group, robust, solver, sparse, weight):
 def _family_residuals(input, params):
     """Row-wise residuals of the family the shapes point at, from the *original* (unsorted) inputs with ordinary
     LieTensor ops — an independent restatement used only to verify a user module at recognition time."""
-    T = LieTensor(params[0].detach(), ltype=SE3_type)
+    T = LieTensor(params[0].detach(), ltype=params[0].ltype)      # SE3, or Sim3 for the Sim3 pose graph
     if len(params) == 2:                                          # bundle adjustment
         obs, ci, pi_ = input
         y = T[ci.long()].Act(params[1].detach()[pi_.long()])
@@ -857,9 +921,10 @@ def _same_residuals(model, input, params, shape, group, trials=2, roles=None):
             for trial in range(trials):
                 if trial:                                         # move off the initial point (small left retraction / shift)
                     for p, s0 in zip(params, saved):
-                        noise = (0.05 * torch.randn(s0.shape[:-1] + ((6,) if isinstance(p, LieTensor) else s0.shape[-1:]),
+                        lie = isinstance(p, LieTensor)
+                        noise = (0.05 * torch.randn(s0.shape[:-1] + (p.ltype.manifold if lie else s0.shape[-1:]),
                                                     generator=gen, dtype=torch.float64)).to(s0.device, s0.dtype)
-                        new = _retract_generic(noise, s0) if isinstance(p, LieTensor) else s0 + noise
+                        new = _retract_generic(noise, s0, p.ltype) if lie else s0 + noise
                         _copy_param(p, new)
                 out = model(*input)
                 if not torch.is_tensor(out) or isinstance(out, LieTensor) or tuple(out.shape) != tuple(shape):
@@ -882,9 +947,9 @@ def _same_residuals(model, input, params, shape, group, trials=2, roles=None):
     return ok
 
 
-def _retract_generic(D, poses):
+def _retract_generic(D, poses, ltype=SE3_type):
     """Exp(D) * poses through the LieTensor ops (any device; recognition time only)."""
-    return (LieTensor(D, ltype=_lt.se3_type).Exp() * LieTensor(poses, ltype=SE3_type)).tensor()
+    return (LieTensor(D, ltype=ltype.dual).Exp() * LieTensor(poses, ltype=ltype)).tensor()
 
 
 def _is_builtin(model, cls):
@@ -906,6 +971,8 @@ def _pgo_weight(weight, input):
 def recognize(model, input, params, group=None, robust=(0, 1.0), solver=None, sparse=False, weight=None):
     """Return a structured problem for (model, input) or None (-> generic dense route)."""
     params = [p for p in params if p.requires_grad]
+    if len(params) == 1 and getattr(params[0], 'ltype', None) is Sim3_type:
+        return _recognize_sim3(model, input, params, group, robust, solver, sparse, weight)
     if weight is not None and not _pgo_weight(weight, input):
         return None
     from ..module.ba import BundleAdjustment
