@@ -354,6 +354,51 @@ LM_OPS += [
 ]
 
 
+# SO3 pose graphs / rotation averaging (csrc/so3pgo.cu + the pcg2.cu kernels at block width 3): r = Log(Z^-1 A^-1 B) on SO3
+# nodes, 3 unknowns per node, J = so3_Jl_inv(r) R(Z^-1 A^-1) (operation.py:23-32).  Slots are 8 words: 6 packed + 2 padding.
+LM_OPS += [
+    ("b200_lm_so3pgo_linearize",
+     [("const REAL*", "nodes", "(N,4) SO3"), ("const REAL*", "Z", "(E,4) SO3"), ("const int*", "ei", "(E)"), ("const int*", "ej", "(E)"),
+      ("const int*", "epos_i", "(E) slot of the edge in its first node's list"),
+      ("const int*", "epos_j", "(E) slot in its second node's list"),
+      ("REAL*", "Mn", "(2E,8) node-ordered blocks: upper triangle of J^T J (6 words, 2 zero words), written at both slots"),
+      ("REAL*", "un", "(2E,3) -J^T r at the first node's slot, +J^T r at the second's"),
+      ("double*", "ws", "ws[0] = sum rho(|r|^2)"), ("int", "robust", ""), ("double", "delta", "")],
+     "modjac + J^T J of optimizer.py:645-656 for the SO3 pose graph (examples/module/pgo/pgo.py:15-25 on SO3 nodes), "
+     "written in node order (no atomics downstream)"),
+    ("b200_lm_so3pgo_loss",
+     [("const REAL*", "nodes", "(N,4)"), ("const REAL*", "Z", "(E,4)"), ("const int*", "ei", "(E)"), ("const int*", "ej", "(E)"),
+      ("double*", "ws", "ws[0] = sum rho(|r|^2)"), ("int", "robust", ""), ("double", "delta", "")],
+     "RobustModel.loss of the SO3 pose graph, optimizer.py:118-125"),
+    ("b200_lm_so3pgo_node_sums",
+     [("const REAL*", "Mn", "(2E,8)"), ("const REAL*", "un", "(2E,3)"), ("const int*", "nptr", "(N+1) offsets per node"),
+      ("REAL*", "Hd", "(N,6) diagonal blocks of J^T J"), ("REAL*", "g", "(N,3) J^T R")],
+     "b200_lm_pgo2_node_sums at block width 3"),
+    ("b200_lm_so3pgo_damp_inv",
+     [("const REAL*", "H", "(n,6) packed 3x3 blocks"), ("double", "scale", "prod(1+damping) over trials"),
+      ("double", "dmin", "diag clamp min"), ("double", "dmax", "diag clamp max"), ("REAL*", "Hd", "(n,6) damped blocks or NULL"),
+      ("REAL*", "extra", "(n,3) amount added to the diagonal, or NULL"),
+      ("REAL*", "Minv", "(n,6) inverses of the damped blocks or NULL")],
+     "clamp + cumulative damping of the diagonal (optimizer.py:657/666) on 3x3 SO3 node blocks"),
+    ("b200_lm_so3pgo_pcg",
+     [("const REAL*", "Mn", "(2E,8) node-ordered blocks"), ("const int*", "nother", "(2E) opposite node of each slot"),
+      ("const int*", "nptr", "(n+1)"), ("const REAL*", "Minv", "(n,6) block-Jacobi preconditioner"),
+      ("const REAL*", "extra", "(n,3) clamp / damping added to diag H"), ("const REAL*", "g", "(n,3); solves (H+extra) x = -g"),
+      ("REAL*", "x", "(n,3)"), ("REAL*", "r", "(n,3)"), ("REAL*", "z", "(n,3)"), ("REAL*", "p0", "(n,3) direction, even iterations"),
+      ("REAL*", "p1", "(n,3) direction, odd iterations"), ("REAL*", "q", "(n,3)"), ("REAL*", "xbest", "(n,3)"),
+      ("double*", "cg", "(16) state, see b200_lm_pgo_pcg"), ("double*", "ws", ""), ("double", "tol", ""),
+      ("long long", "maxiter", ""), ("long long", "first_iter", ""), ("long long", "iters", "")],
+     "b200_lm_pgo2_pcg at block width 3: PCG.forward loop, optim/solver.py:312-340, no atomics, bit-reproducible"),
+    ("b200_lm_so3pgo_cg_finish",
+     [("REAL*", "x", "(n,3)"), ("const REAL*", "xbest", "(n,3)"), ("const double*", "cg", "(16) state")],
+     "x <- best iterate unless the PCG converged (the best-iterate guard of b200_lm_cg_finish at width 3)"),
+    ("b200_lm_so3pgo_predicted",
+     [("const REAL*", "Mn", "(2E,8)"), ("const int*", "nother", "(2E)"), ("const int*", "nptr", "(n+1)"), ("const REAL*", "x", "(n,3) step"),
+      ("const REAL*", "g", "(n,3)"), ("double*", "ws", "ws[0] = x^T H x + 2 x^T g")],
+     "TrustRegion 'predicted' reduction of the SO3 pose graph, optim/strategy.py:143, by gather"),
+]
+
+
 LM_OPS += [
     ("b200_lm_reproj2_accum",
      [("const REAL*", "nodes", "(N,7) SE3 poses"), ("const REAL*", "pts", "(m,3) points in the frame of pose a, rows sorted by pair"),

@@ -6,6 +6,7 @@
 // calling the library's own entry points back to back, and the two things the host must learn — "has
 // the CG finished?" and "was the trial accepted?" — arrive through mapped pinned memory that small kernels publish into.
 #include <string.h>
+#include <type_traits>
 #include "lm_common.cuh"
 #include "b200pose.h"
 
@@ -62,27 +63,49 @@ template <typename CT> struct Api;
     static constexpr auto predicted = b200_lm_pgo2_predicted_##SFX;                                                   \
     static constexpr auto exp = b200_se3_exp_fwd_##SFX;                                                               \
     static constexpr auto mul = b200_SE3_mul_fwd_##SFX;                                                               \
-    static constexpr auto loss0 = b200_lm_pgo_loss_##SFX;                                                             \
+    static constexpr auto loss = b200_lm_pgo_loss_##SFX;                                                              \
     static constexpr auto loss1 = b200_lm_reproj2_loss_##SFX;                                                         \
   };
 B200_API(f32, float)
 B200_API(f64, double)
-// family 2 (Sim3 pose graph): the same sequence at block width 7 (entry points of the same signatures)
-template <typename CT> struct Sim3Api;
-#define B200_SIM3_API(SFX, CT)                                                                                        \
-  template <> struct Sim3Api<CT> {                                                                                    \
-    static constexpr auto linearize = b200_lm_sim3pgo_linearize_##SFX;                                                \
-    static constexpr auto node_sums = b200_lm_sim3pgo_node_sums_##SFX;                                                \
-    static constexpr auto damp_inv = b200_lm_sim3pgo_damp_inv_##SFX;                                                  \
-    static constexpr auto pcg = b200_lm_sim3pgo_pcg_##SFX;                                                            \
-    static constexpr auto finish = b200_lm_sim3pgo_cg_finish_##SFX;                                                   \
-    static constexpr auto predicted = b200_lm_sim3pgo_predicted_##SFX;                                                \
-    static constexpr auto exp = b200_sim3_exp_fwd_##SFX;                                                              \
-    static constexpr auto mul = b200_Sim3_mul_fwd_##SFX;                                                              \
-    static constexpr auto loss = b200_lm_sim3pgo_loss_##SFX;                                                          \
+// families 2 (Sim3 pose graph) and 3 (SO3 pose graph): the same sequence at block widths 7 and 3 (entry points of the
+// same signatures)
+#define B200_LIE_PGO_API(NAME, PFX, GRP, ALG, SFX, CT)                                                                \
+  template <> struct NAME<CT> {                                                                                       \
+    static constexpr auto linearize = b200_lm_##PFX##_linearize_##SFX;                                                \
+    static constexpr auto node_sums = b200_lm_##PFX##_node_sums_##SFX;                                                \
+    static constexpr auto damp_inv = b200_lm_##PFX##_damp_inv_##SFX;                                                  \
+    static constexpr auto pcg = b200_lm_##PFX##_pcg_##SFX;                                                            \
+    static constexpr auto finish = b200_lm_##PFX##_cg_finish_##SFX;                                                   \
+    static constexpr auto predicted = b200_lm_##PFX##_predicted_##SFX;                                                \
+    static constexpr auto exp = b200_##ALG##_exp_fwd_##SFX;                                                           \
+    static constexpr auto mul = b200_##GRP##_mul_fwd_##SFX;                                                           \
+    static constexpr auto loss = b200_lm_##PFX##_loss_##SFX;                                                          \
   };
-B200_SIM3_API(f32, float)
-B200_SIM3_API(f64, double)
+template <typename CT> struct Sim3Api;
+template <typename CT> struct So3Api;
+B200_LIE_PGO_API(Sim3Api, sim3pgo, Sim3, sim3, f32, float)
+B200_LIE_PGO_API(Sim3Api, sim3pgo, Sim3, sim3, f64, double)
+B200_LIE_PGO_API(So3Api, so3pgo, SO3, so3, f32, float)
+B200_LIE_PGO_API(So3Api, so3pgo, SO3, so3, f64, double)
+
+// the entry points and widths of the family being run: W unknowns per node, parameter width D
+template <typename CT> struct PgoFns {
+  template <class F> using Fn = std::remove_cv_t<F>;
+  Fn<decltype(Api<CT>::linearize)> linearize;             // families 0, 2 and 3 (family 1: Api::accum2)
+  Fn<decltype(Api<CT>::node_sums)> node_sums;
+  Fn<decltype(Api<CT>::damp_inv)> damp_inv;
+  Fn<decltype(Api<CT>::pcg)> pcg;
+  Fn<decltype(Api<CT>::finish)> finish;
+  Fn<decltype(Api<CT>::predicted)> predicted;
+  Fn<decltype(Api<CT>::exp)> exp;
+  Fn<decltype(Api<CT>::mul)> mul;
+  Fn<decltype(Api<CT>::loss)> loss;                       // families 0, 2 and 3 (family 1: Api::loss1)
+  long long W, D;
+};
+template <typename CT, class F> static PgoFns<CT> pgo_fns(long long W, long long D) {
+  return {F::linearize, F::node_sums, F::damp_inv, F::pcg, F::finish, F::predicted, F::exp, F::mul, F::loss, W, D};
+}
 
 static LmCtl ctl_from(const double* c) {
   LmCtl k;
@@ -94,38 +117,36 @@ static LmCtl ctl_from(const double* c) {
 
 template <typename CT> static int pgo_step(b200_pgo_step_args* a, void* stream) {
   using A = Api<CT>;
-  using S = Sim3Api<CT>;
   cudaStream_t s = (cudaStream_t)stream;
   const long long N = a->N, E = a->E;
-  const bool sim3 = a->family == 2;
-  const long long W = sim3 ? 7 : 6, D = sim3 ? 8 : 7;      // unknowns per node, parameter width
+  const PgoFns<CT> f = a->family == 2   ? pgo_fns<CT, Sim3Api<CT>>(7, 8)
+                       : a->family == 3 ? pgo_fns<CT, So3Api<CT>>(3, 4)
+                                        : pgo_fns<CT, A>(6, 7);
+  const bool reproj2 = a->family == 1;
   CT* nodes = (CT*)a->nodes;
   CT *Mn = (CT*)a->Mn, *un = (CT*)a->un, *Hd = (CT*)a->Hd, *g = (CT*)a->g, *extra = (CT*)a->extra, *Minv = (CT*)a->Minv;
   CT *x = (CT*)a->x, *r = (CT*)a->r, *z = (CT*)a->z, *p0 = (CT*)a->p0, *p1 = (CT*)a->p1, *q = (CT*)a->q, *xbest = (CT*)a->xbest;
   CT *X7 = (CT*)a->X7, *Pt = (CT*)a->Pt;
   volatile double* host = a->host;
   if (!a->retry) {                                       // linearise at the current parameters (kept across rejected trials)
-    if (a->family == 0)
-      B200_TRY(A::linearize(nodes, (const CT*)a->Z, a->ei, a->ej, a->epos_i, a->epos_j, Mn, un, a->ws3, a->robust, a->delta, E, stream));
-    else if (sim3)
-      B200_TRY(S::linearize(nodes, (const CT*)a->Z, a->ei, a->ej, a->epos_i, a->epos_j, Mn, un, a->ws3, a->robust, a->delta, E, stream));
-    else
+    if (reproj2)
       B200_TRY(A::accum2(nodes, (const CT*)a->pts, (const CT*)a->pix, a->pseg, a->pa, a->pb, a->intr, a->epos_i, a->epos_j, Mn, un,
                          a->ws3, a->robust, a->delta, E, stream));
-    B200_TRY((sim3 ? S::node_sums : A::node_sums)(Mn, un, a->nptr, Hd, g, N, stream));
+    else
+      B200_TRY(f.linearize(nodes, (const CT*)a->Z, a->ei, a->ej, a->epos_i, a->epos_j, Mn, un, a->ws3, a->robust, a->delta, E, stream));
+    B200_TRY(f.node_sums(Mn, un, a->nptr, Hd, g, N, stream));
   }
-  B200_TRY((sim3 ? S::damp_inv : A::damp_inv)(Hd, a->scale, a->dmin, a->dmax, (CT*)nullptr, extra, Minv, N, stream));
+  B200_TRY(f.damp_inv(Hd, a->scale, a->dmin, a->dmax, (CT*)nullptr, extra, Minv, N, stream));
   // PCG: chunks of iterations without host involvement; after each chunk a one-thread kernel publishes the CG state
-  const long long maxiter = a->maxiter > 0 ? a->maxiter : 10 * W * N;
-  const auto pcg = sim3 ? S::pcg : A::pcg;
+  const long long maxiter = a->maxiter > 0 ? a->maxiter : 10 * f.W * N;
   long long it = 0;
   double cgseq = host[32];
   for (;;) {
     long long n = (it == 0 && a->hint > 0) ? a->hint : 8;
     if (n > maxiter - it) n = maxiter - it;
     if (n < 1) n = 1;
-    B200_TRY(pcg(Mn, a->nother, a->nptr, Minv, extra, g, x, r, z, p0, p1, q, xbest, a->cg, a->ws0, a->tol, maxiter, it, n, N,
-                 stream));
+    B200_TRY(f.pcg(Mn, a->nother, a->nptr, Minv, extra, g, x, r, z, p0, p1, q, xbest, a->cg, a->ws0, a->tol, maxiter, it, n, N,
+                   stream));
     it += n;
     cgseq += 1.0;
     publish_kernel<<<1, 32, 0, s>>>(a->cg, 16, a->host + 16, cgseq);
@@ -134,16 +155,15 @@ template <typename CT> static int pgo_step(b200_pgo_step_args* a, void* stream) 
     if (host[16 + 5] != 0.0 || it >= maxiter) break;      // done flag of the CG state
   }
   a->iters_out = (long long)host[16 + 6];
-  B200_TRY((sim3 ? S::finish : A::finish)(x, xbest, a->cg, N, stream));
-  B200_TRY((sim3 ? S::predicted : A::predicted)(Mn, a->nother, a->nptr, x, g, a->ws2, N, stream));
-  B200_TRY((sim3 ? S::exp : A::exp)(x, X7, N, stream));  // retraction P' = Exp(D) P  (lietensor.py:442-444)
-  B200_TRY((sim3 ? S::mul : A::mul)(X7, nodes, Pt, N, stream));
-  if (a->family == 0) B200_TRY(A::loss0(Pt, (const CT*)a->Z, a->ei, a->ej, a->ws1, a->robust, a->delta, E, stream));
-  else if (sim3) B200_TRY(S::loss(Pt, (const CT*)a->Z, a->ei, a->ej, a->ws1, a->robust, a->delta, E, stream));
-  else B200_TRY(A::loss1(Pt, (const CT*)a->pts, (const CT*)a->pix, a->pseg, a->pa, a->pb, a->intr, a->ws1, a->robust, a->delta, E, stream));
+  B200_TRY(f.finish(x, xbest, a->cg, N, stream));
+  B200_TRY(f.predicted(Mn, a->nother, a->nptr, x, g, a->ws2, N, stream));
+  B200_TRY(f.exp(x, X7, N, stream));                     // retraction P' = Exp(D) P  (lietensor.py:442-444)
+  B200_TRY(f.mul(X7, nodes, Pt, N, stream));
+  if (reproj2) B200_TRY(A::loss1(Pt, (const CT*)a->pts, (const CT*)a->pix, a->pseg, a->pa, a->pb, a->intr, a->ws1, a->robust, a->delta, E, stream));
+  else B200_TRY(f.loss(Pt, (const CT*)a->Z, a->ei, a->ej, a->ws1, a->robust, a->delta, E, stream));
   host[ST_SIZE - 1] = -1.0;
   pgo_decide_kernel<<<1, 32, 0, s>>>(a->ws3, a->ws1, a->ws2, ctl_from(a->ctl), a->st, a->host, (double)a->seq);
-  commit_kernel<CT><<<lm_grid(N * D, kLmThreads), kLmThreads, 0, s>>>(a->st, Pt, nodes, N * D);
+  commit_kernel<CT><<<lm_grid(N * f.D, kLmThreads), kLmThreads, 0, s>>>(a->st, Pt, nodes, N * f.D);
   B200_TRY((int)cudaGetLastError());
   return spin_until(host + (ST_SIZE - 1), (double)a->seq, s);
 }
@@ -251,6 +271,7 @@ B200_EXPORT long long b200_ba_step_args_size(void) { return (long long)sizeof(b2
 
 B200_EXPORT int b200_lm_pgo2_step(b200_pgo_step_args* args, void* stream) {
   if (!args || args->N <= 0) return 0;
+  if (args->family < 0 || args->family > 3) return (int)cudaErrorInvalidValue;
   return args->is64 ? b200pose::pgo_step<double>(args, stream) : b200pose::pgo_step<float>(args, stream);
 }
 B200_EXPORT long long b200_pgo_step_args_size(void) { return (long long)sizeof(b200_pgo_step_args); }

@@ -18,7 +18,8 @@ namespace b200pose {
 
 
 // diag <- clamp(diag, dmin, dmax) * scale (optimizer.py:657 + cumulative :666); optional outputs: the damped block,
-// the amount added to the diagonal, the inverse of the damped block.  W = 6: SE3 blocks; W = 7: Sim3 pose-graph blocks.
+// the amount added to the diagonal, the inverse of the damped block.  W = 6: SE3 blocks; W = 7: Sim3 pose-graph blocks;
+// W = 3: SO3 pose-graph blocks.
 template <int W, typename T> __device__ __forceinline__ void blkw_unpack(const T* a, T (&A)[W][W]) {
   if constexpr (W == 6) sym6_unpack(a, A);
   else symn_unpack<T, W>(a, A);
@@ -201,6 +202,8 @@ PCG_LAUNCH_INST(float, 6)
 PCG_LAUNCH_INST(double, 6)
 PCG_LAUNCH_INST(float, 7)
 PCG_LAUNCH_INST(double, 7)
+PCG_LAUNCH_INST(float, 3)
+PCG_LAUNCH_INST(double, 3)
 
 }  // namespace b200pose
 
@@ -306,6 +309,18 @@ static int ba_pcg_run(const CT* Y4, const CT* poses, const int* pidx, const int*
                                                   void* stream) {                                                     \
     if (n <= 0) return 0;                                                                                             \
     LM_LAUNCH(cg_finish_kernel<CT>, n * 7, stream, x, xbest, cg, n * 7);                                              \
+    return (int)cudaGetLastError();                                                                                   \
+  }                                                                                                                   \
+  B200_EXPORT int b200_lm_so3pgo_damp_inv_##SFX(const CT* H, double scale, double dmin, double dmax, CT* Hd,          \
+                                                CT* extra, CT* Minv, long long n, void* stream) {                     \
+    if (n <= 0) return 0;                                                                                             \
+    LM_LAUNCH((blkw_damp_inv_kernel<CT, 3>), n, stream, H, (CT)scale, (CT)dmin, (CT)dmax, Hd, extra, Minv, n);        \
+    return (int)cudaGetLastError();                                                                                   \
+  }                                                                                                                   \
+  B200_EXPORT int b200_lm_so3pgo_cg_finish_##SFX(CT* x, const CT* xbest, const double* cg, long long n,               \
+                                                 void* stream) {                                                      \
+    if (n <= 0) return 0;                                                                                             \
+    LM_LAUNCH(cg_finish_kernel<CT>, n * 3, stream, x, xbest, cg, n * 3);                                              \
     return (int)cudaGetLastError();                                                                                   \
   }                                                                                                                   \
   B200_EXPORT int b200_lm_pt3_damp_inv_##SFX(const CT* H, double scale, double dmin, double dmax, CT* Hinv,           \

@@ -12,7 +12,8 @@
 //        A:  p' = z + beta p;  q = (H + D) p';  p'.q            (gather over node-ordered blocks)
 //        B:  alpha;  x += alpha p';  r -= alpha q;  z = M^-1 r;  r.z, r.r;  stop / best-iterate bookkeeping
 //    i.e. 2 launches per iteration instead of 4, same arithmetic as optim/solver.py:312-340 with M = block-Jacobi.
-// The kernels are templated on the block width W: 6 for SE3 nodes, 7 for Sim3 nodes (sim3pgo.cu; 28-word slots).
+// The kernels are templated on the block width W: 6 for SE3 nodes, 7 for Sim3 nodes (sim3pgo.cu; 28-word slots), 3 for
+// SO3 nodes (so3pgo.cu; 8-word slots).
 #include "lm_common.cuh"
 #include "sim3pgo_math.cuh"
 
@@ -21,10 +22,11 @@ namespace b200pose {
 enum { CG2_RZ0 = 0, CG2_RZ1 = 1, CG2_PQ = 2, CG2_DONE = 5 };       // same slots as pcg.cu
 constexpr int kLanes = 4;                                           // lanes cooperating on one node
 // node-ordered slot of W unknowns: W = 6 (SE3): 21 words padded to 24 (96 / 192 B, six 16-byte loads in fp32);
-// W = 7 (Sim3, sim3pgo.cu): 28 words, unpadded (112 / 224 B)
+// W = 7 (Sim3, sim3pgo.cu): 28 words, unpadded (112 / 224 B); W = 3 (SO3, so3pgo.cu): 6 words padded to 8 (32 / 64 B)
 template <int W> struct Slot;
 template <> struct Slot<6> { static constexpr int words = 24, packed = 21; };
 template <> struct Slot<7> { static constexpr int words = 28, packed = 28; };
+template <> struct Slot<3> { static constexpr int words = 8, packed = 6; };
 
 template <typename T, int NW> __device__ __forceinline__ void ld_slot(const T* __restrict__ p, T (&a)[NW]) {
   if (sizeof(T) == 4) {
@@ -59,7 +61,7 @@ template <typename T> struct Pair6g;
 template <> struct Pair6g<float> { using type = float2; };
 template <> struct Pair6g<double> { using type = double2; };
 // gather of one node's six values as three 8- / 16-byte pairs (see pcg.cu ld6): half the LSU wavefronts of scalar loads;
-// a node's seven values are not pair-aligned and are read value by value
+// a node's seven (or three) values are not pair-aligned and are read value by value
 template <typename T, int W> __device__ __forceinline__ void ldwg(const T* __restrict__ p, long long i, T (&v)[W]) {
   if constexpr (W == 6) {
     using P = typename Pair6g<T>::type;
@@ -216,7 +218,8 @@ static int pgo2_predicted_launch(const CT* Mn, const int* nother, const int* npt
 
 using namespace b200pose;
 
-// W = 6: SE3 pose graphs and pose pairs (vectors accessed as pairs, so they must be pair-aligned); W = 7: Sim3 pose graphs
+// W = 6: SE3 pose graphs and pose pairs (vectors accessed as pairs, so they must be pair-aligned); W = 7: Sim3 pose graphs;
+// W = 3: SO3 pose graphs
 #define PCG2_ABI(SFX, CT)                                                                                             \
   B200_EXPORT int b200_lm_pgo2_node_sums_##SFX(const CT* Mn, const CT* un, const int* nptr, CT* Hd, CT* g,            \
                                                long long N, void* stream) {                                           \
@@ -251,6 +254,21 @@ using namespace b200pose;
   B200_EXPORT int b200_lm_sim3pgo_predicted_##SFX(const CT* Mn, const int* nother, const int* nptr, const CT* x,      \
                                                   const CT* g, double* ws, long long n, void* stream) {               \
     return pgo2_predicted_launch<CT, 7>(Mn, nother, nptr, x, g, ws, n, (cudaStream_t)stream);                         \
+  }                                                                                                                   \
+  B200_EXPORT int b200_lm_so3pgo_node_sums_##SFX(const CT* Mn, const CT* un, const int* nptr, CT* Hd, CT* g,          \
+                                                 long long N, void* stream) {                                         \
+    return pgo2_node_sums_launch<CT, 3>(Mn, un, nptr, Hd, g, N, (cudaStream_t)stream);                                \
+  }                                                                                                                   \
+  B200_EXPORT int b200_lm_so3pgo_pcg_##SFX(const CT* Mn, const int* nother, const int* nptr, const CT* Minv,          \
+                                           const CT* extra, const CT* g, CT* x, CT* r, CT* z, CT* p0, CT* p1, CT* q,  \
+                                           CT* xbest, double* cg, double* ws, double tol, long long maxiter,          \
+                                           long long first_iter, long long iters, long long n, void* stream) {        \
+    return pgo2_pcg_run<CT, 3>(Mn, nother, nptr, Minv, extra, g, x, r, z, p0, p1, q, xbest, cg, ws, tol, maxiter,     \
+                               first_iter, iters, n, (cudaStream_t)stream);                                           \
+  }                                                                                                                   \
+  B200_EXPORT int b200_lm_so3pgo_predicted_##SFX(const CT* Mn, const int* nother, const int* nptr, const CT* x,       \
+                                                 const CT* g, double* ws, long long n, void* stream) {                \
+    return pgo2_predicted_launch<CT, 3>(Mn, nother, nptr, x, g, ws, n, (cudaStream_t)stream);                         \
   }
 
 PCG2_ABI(f32, float)

@@ -4,6 +4,7 @@ Like the Lie ops, only the CUDA dispatch key has a kernel.  All host-visible sca
 a small fp64 tensor on the device (`sums`), so the caller decides when to synchronise.
 """
 import ctypes
+from typing import NamedTuple
 
 import torch
 from torch import Tensor
@@ -323,59 +324,74 @@ def _run_chunks(enqueue, cg, maxiter, hint=0):
             return int(st[6])
 
 
+class NodeWidth(NamedTuple):
+    """One block width W of the node-ordered route (csrc/pcg2.cu Slot<W>): words per slot, packed words of a W x W block,
+    parameter width D of a node and the width-specific entry points."""
+    slot: int
+    packed: int
+    D: int
+    node_sums: str
+    damp_inv: str
+    pcg: str
+    cg_finish: str
+    predicted: str
+
+
+# W = 6: SE3 pose graphs and pose pairs; 7: Sim3 pose graphs; 3: SO3 pose graphs (include/b200pose.h, b200_pgo_step_args)
+NODE_WIDTHS = {
+    6: NodeWidth(24, 21, 7, "b200_lm_pgo2_node_sums", "b200_lm_blk6_damp_inv", "b200_lm_pgo2_pcg", "b200_lm_cg_finish",
+                 "b200_lm_pgo2_predicted"),
+    7: NodeWidth(28, 28, 8, "b200_lm_sim3pgo_node_sums", "b200_lm_sim3pgo_damp_inv", "b200_lm_sim3pgo_pcg",
+                 "b200_lm_sim3pgo_cg_finish", "b200_lm_sim3pgo_predicted"),
+    3: NodeWidth(8, 6, 4, "b200_lm_so3pgo_node_sums", "b200_lm_so3pgo_damp_inv", "b200_lm_so3pgo_pcg",
+                 "b200_lm_so3pgo_cg_finish", "b200_lm_so3pgo_predicted"),
+}
+# block width and node-ordered linearisation of each problem kind with edges (ei, ej, Z); "reproj2" is linearised by pose pair
+KIND_WIDTH = {"pgo": 6, "reproj2": 6, "sim3": 7, "so3": 3}
+_EDGE_LINEARIZE = {"pgo": "b200_lm_pgo_linearize_n", "sim3": "b200_lm_sim3pgo_linearize", "so3": "b200_lm_so3pgo_linearize"}
+
+
 def pgo_linearize_nodes(kind, prob, nodes, robust, delta):
-    """Blocks of the current linearisation directly in node order (csrc/lm.cu store_edge_blocks, csrc/sim3pgo.cu) and, by
-    gather, the diagonal blocks Hd and J^T R.  kind: "pgo" (Log(Z^-1 A^-1 B) edges), "reproj2" (pose pairs) or "sim3"
-    (Log(Z^-1 A^-1 B) on Sim3 nodes: 7 unknowns per node, 28-word slots)."""
+    """Blocks of the current linearisation directly in node order (csrc/lm.cu store_edge_blocks, csrc/sim3pgo.cu,
+    csrc/so3pgo.cu) and, by gather, the diagonal blocks Hd and J^T R.  kind: "pgo" (Log(Z^-1 A^-1 B) edges), "reproj2"
+    (pose pairs), "sim3" or "so3" (Log(Z^-1 A^-1 B) on Sim3 / SO3 nodes); its block width is KIND_WIDTH[kind]."""
     E, N = prob.ei.shape[0], prob.nptr.shape[0] - 1
     E2 = 2 * E
     dt, dev = nodes.dtype, nodes.device
     ws = _workspace(dev)
-    W, slot, pw = (7, 28, 28) if kind == "sim3" else (6, 24, 21)
-    Mn, un = torch.empty(E2, slot, dtype=dt, device=dev), torch.empty(E2, W, dtype=dt, device=dev)
-    if kind == "pgo":
-        _launch("b200_lm_pgo_linearize_n", nodes, [_p(nodes), _p(prob.Z), _p(prob.ei), _p(prob.ej), _p(prob.epos_i), _p(prob.epos_j),
-                                                   _p(Mn), _p(un), _p(ws), int(robust), float(delta)], E)
-    elif kind == "sim3":
-        _launch("b200_lm_sim3pgo_linearize", nodes, [_p(nodes), _p(prob.Z), _p(prob.ei), _p(prob.ej), _p(prob.epos_i),
-                                                     _p(prob.epos_j), _p(Mn), _p(un), _p(ws), int(robust), float(delta)], E)
-    else:
+    W = KIND_WIDTH[kind]
+    spec = NODE_WIDTHS[W]
+    Mn, un = torch.empty(E2, spec.slot, dtype=dt, device=dev), torch.empty(E2, W, dtype=dt, device=dev)
+    if kind == "reproj2":
         k = (ctypes.c_double * 5)(*prob.intr)
         _launch("b200_lm_reproj2_accum_n", nodes, [_p(nodes), _p(prob.pts), _p(prob.pix), _p(prob.pseg), _p(prob.pa), _p(prob.pb),
                                                    ctypes.addressof(k), _p(prob.epos_i), _p(prob.epos_j), _p(Mn), _p(un), _p(ws),
                                                    int(robust), float(delta)], E)
-    cur = ws[:1].clone()
-    Hd, g = torch.empty(N, pw, dtype=dt, device=dev), torch.empty(N, W, dtype=dt, device=dev)
-    if kind == "sim3":
-        _launch("b200_lm_sim3pgo_node_sums", nodes, [_p(Mn), _p(un), _p(prob.nptr), _p(Hd), _p(g)], N)
     else:
-        _launch("b200_lm_pgo2_node_sums", nodes, [_p(Mn), _p(un), _p(prob.nptr), _p(Hd), _p(g)], N)
+        _launch(_EDGE_LINEARIZE[kind], nodes, [_p(nodes), _p(prob.Z), _p(prob.ei), _p(prob.ej), _p(prob.epos_i), _p(prob.epos_j),
+                                               _p(Mn), _p(un), _p(ws), int(robust), float(delta)], E)
+    cur = ws[:1].clone()
+    Hd, g = torch.empty(N, spec.packed, dtype=dt, device=dev), torch.empty(N, W, dtype=dt, device=dev)
+    _launch(spec.node_sums, nodes, [_p(Mn), _p(un), _p(prob.nptr), _p(Hd), _p(g)], N)
     return Mn, Hd, g, cur
 
 
 def pgo_solve_nodes(Mn, nother, nptr, Hd, g, scale, dmin, dmax, tol, maxiter, hint=0):
     """(H + clamp/damping) x = -g on node-ordered blocks (csrc/pcg2.cu): two launches per iteration, no atomics.
-    The block width W (6: SE3 nodes, 7: Sim3 nodes) is g's.  Returns x (n,W), iterations, predicted (1,) fp64 on device."""
+    The block width W (NODE_WIDTHS) is g's.  Returns x (n,W), iterations, predicted (1,) fp64 on device."""
     dev, dt, n, W = Mn.device, Mn.dtype, Hd.shape[0], g.shape[1]
+    spec = NODE_WIDTHS[W]
     ws, cg = _workspace(dev), _cg(dev)
     extra = torch.empty(n, W, dtype=dt, device=dev)
     Minv = torch.empty_like(Hd)
     x, r, z, p0, p1, q, xbest = (torch.empty(n, W, dtype=dt, device=dev) for _ in range(7))
     maxiter = int(maxiter) if maxiter is not None else 10 * W * n
-    if W == 7:
-        _launch("b200_lm_sim3pgo_damp_inv", Mn, [_p(Hd), float(scale), float(dmin), float(dmax), _p(None), _p(extra), _p(Minv)], n)
-        iters = _run_chunks(lambda it0, k: _launch("b200_lm_sim3pgo_pcg", Mn, [
-            _p(Mn), _p(nother), _p(nptr), _p(Minv), _p(extra), _p(g), _p(x), _p(r), _p(z), _p(p0), _p(p1), _p(q), _p(xbest),
-            _p(cg), _p(ws), float(tol), maxiter, it0, k], n), cg, maxiter, hint)
-        _launch("b200_lm_sim3pgo_cg_finish", Mn, [_p(x), _p(xbest), _p(cg)], n)
-        _launch("b200_lm_sim3pgo_predicted", Mn, [_p(Mn), _p(nother), _p(nptr), _p(x), _p(g), _p(ws)], n)
-        return x, iters, ws[:1].clone()
-    _launch("b200_lm_blk6_damp_inv", Mn, [_p(Hd), float(scale), float(dmin), float(dmax), _p(None), _p(extra), _p(Minv)], n)
-    iters = _run_chunks(lambda it0, k: _launch("b200_lm_pgo2_pcg", Mn, [
+    _launch(spec.damp_inv, Mn, [_p(Hd), float(scale), float(dmin), float(dmax), _p(None), _p(extra), _p(Minv)], n)
+    iters = _run_chunks(lambda it0, k: _launch(spec.pcg, Mn, [
         _p(Mn), _p(nother), _p(nptr), _p(Minv), _p(extra), _p(g), _p(x), _p(r), _p(z), _p(p0), _p(p1), _p(q), _p(xbest),
         _p(cg), _p(ws), float(tol), maxiter, it0, k], n), cg, maxiter, hint)
-    _launch("b200_lm_cg_finish", Mn, [_p(x), _p(xbest), _p(cg)], n)
-    _launch("b200_lm_pgo2_predicted", Mn, [_p(Mn), _p(nother), _p(nptr), _p(x), _p(g), _p(ws)], n)
+    _launch(spec.cg_finish, Mn, [_p(x), _p(xbest), _p(cg)], n)
+    _launch(spec.predicted, Mn, [_p(Mn), _p(nother), _p(nptr), _p(x), _p(g), _p(ws)], n)
     return x, iters, ws[:1].clone()
 
 
@@ -384,6 +400,14 @@ def sim3pgo_loss(nodes, Z, ei, ej, robust=0, delta=1.0):
     nodes, Z = _same(nodes, Z)
     ws = _workspace(nodes.device)
     _launch("b200_lm_sim3pgo_loss", nodes, [_p(nodes), _p(Z), _p(ei), _p(ej), _p(ws), int(robust), float(delta)], Z.shape[0])
+    return ws[:1].clone()
+
+
+def so3pgo_loss(nodes, Z, ei, ej, robust=0, delta=1.0):
+    """(1,) fp64 device tensor: sum rho(|r|^2) of the SO3 pose graph at the given (N,4) nodes."""
+    nodes, Z = _same(nodes, Z)
+    ws = _workspace(nodes.device)
+    _launch("b200_lm_so3pgo_loss", nodes, [_p(nodes), _p(Z), _p(ei), _p(ej), _p(ws), int(robust), float(delta)], Z.shape[0])
     return ws[:1].clone()
 
 

@@ -182,9 +182,9 @@ class PgoDeviceStep:
         N, E = nodes.shape[0], prob.ei.shape[0]
         self.device, self.dtype, self.comm = dev, dt, None
         new = lambda *shape: torch.empty(*shape, dtype=dt, device=dev)
-        family = {"pgo": 0, "reproj2": 1, "sim3": 2}[prob.kind]
-        # block width W, slot words, packed block words and parameter width D of the family (include/b200pose.h)
-        W, slot, pw, D = (7, 28, 28, 8) if family == 2 else (6, 24, 21, 7)
+        family = {"pgo": 0, "reproj2": 1, "sim3": 2, "so3": 3}[prob.kind]
+        W = _fused.KIND_WIDTH[prob.kind]
+        slot, pw, D = _fused.NODE_WIDTHS[W][:3]         # slot words, packed block words, parameter width (include/b200pose.h)
         self.buf = {"Mn": new(2 * E, slot), "un": new(2 * E, W), "Hd": new(N, pw), "g": new(N, W), "extra": new(N, W),
                     "Minv": new(N, pw), "x": new(N, W), "r": new(N, W), "z": new(N, W), "p0": torch.zeros(N, W, dtype=dt, device=dev),
                     "p1": torch.zeros(N, W, dtype=dt, device=dev), "q": new(N, W), "xbest": new(N, W), "X7": new(N, D),

@@ -228,6 +228,10 @@ class LevenbergMarquardt(_SecondOrder):
         self._problem = structured.recognize(self.model.model, input, params, self.group,
                                              self._robust, self.solver, self.sparse, weight)
         if self._problem is None and weight is None and (self.sparse or isinstance(self.solver, CG)):
+            # an SO3 pose graph (rotation averaging) takes its node-ordered route
+            self._problem = structured.recognize_so3_graph(self.model.model, input, params, self.group, self._robust,
+                                                           self.solver, self.sparse, weight)
+        if self._problem is None and weight is None and (self.sparse or isinstance(self.solver, CG)):
             # not one of the fused families: per-residual Jacobian blocks for any batch-separable model of `sjac`
             # parameters (what the reference delegates to `bae`, optimizer.py:629-643)
             from . import blocks

@@ -19,7 +19,7 @@ import torch
 
 from .. import _C
 from ..lietensor import lietensor as _lt
-from ..lietensor.lietensor import LieTensor, Parameter, SE3_type, Sim3_type
+from ..lietensor.lietensor import LieTensor, Parameter, SE3_type, SO3_type, Sim3_type
 from ..lietensor.scan import _sms
 from . import _fused  # noqa: F401  (registers the ops)
 from . import _lmstep
@@ -52,6 +52,12 @@ def _retract_sim3(D, nodes):
     """Exp(D) * nodes for (n,7) steps and (n,8) Sim3 rows (CUDA only: the Sim3 pose-graph route runs on one GPU)."""
     X = _C.launch_rows("b200_sim3_exp_fwd", [D.contiguous()], [8])[0]
     return _C.launch_rows("b200_Sim3_mul_fwd", [X, nodes.contiguous()], [8])[0]
+
+
+def _retract_so3(D, nodes):
+    """Exp(D) * nodes for (n,3) steps and (n,4) SO3 rows (CUDA only: the SO3 pose-graph route runs on one GPU)."""
+    X = _C.launch_rows("b200_so3_exp_fwd", [D.contiguous()], [4])[0]
+    return _C.launch_rows("b200_SO3_mul_fwd", [X, nodes.contiguous()], [4])[0]
 
 
 class _Problem:
@@ -290,7 +296,7 @@ class PGOProblem(_Problem):
     per-edge scatter route (information matrices, or edges sharded over a process group): per-edge M_e = J^T J and
                u_e = J^T r (one kernel), diagonal blocks + gradient by atomics, a matvec that walks the edges
                (csrc/lm.cu lm_pgo_spmv_kernel).  With a group, Hd, g, every matvec and the scalars are all-reduced."""
-    D = 7                       # parameter width of a node (Sim3PGOProblem: 8)
+    D = 7                       # parameter width of a node (Sim3PGOProblem: 8, SO3PGOProblem: 4)
 
     def __init__(self, model, edges, Z, key, group, robust, tol, maxiter, param=None, weight=None):
         self.model, self.key, self.group, self.robust = model, key, group, robust
@@ -488,6 +494,29 @@ class Sim3PGOProblem(PGOProblem):
 
     def _retract(self, D, nodes):
         return _retract_sim3(D, nodes)
+
+
+class SO3PGOProblem(PGOProblem):
+    """SO3 pose graph r_e = Log(Z_e^-1 A^-1 B) on SO3 nodes (examples/module/pgo `PoseGraph` with pp.SO3 nodes): rotation
+    averaging, the first stage of global structure from motion.  A node has 3 unknowns; J = so3_Jl_inv(r) R(Z^-1 A^-1)
+    (csrc/so3pgo_math.cuh).  The blocks are written in node order and solved by the PCG of csrc/pcg2.cu at block width 3;
+    the update is Exp(D) P.  One CUDA device, no process group, no information matrices (those graphs keep the generic
+    route)."""
+    D = 4
+
+    def __init__(self, model, edges, Z, key, robust, tol, maxiter, param=None):
+        super().__init__(model, edges, Z, key, None, robust, tol, maxiter, param=param)
+        self.kind = "so3"
+
+    def _loss_at(self, nodes):
+        return _fused.so3pgo_loss(nodes, self.Z, self.ei, self.ej, *self.robust)
+
+    def linearize(self):
+        Mn, Hd, g, cur = _fused.pgo_linearize_nodes(self.kind, self, self._nodes(), *self.robust)
+        return (Mn,), Hd, g, cur, None
+
+    def _retract(self, D, nodes):
+        return _retract_so3(D, nodes)
 
 
 def _peer_allreduce(prob, param, max_elems):
@@ -832,14 +861,16 @@ def _bal_params_ok(K, T, P):
             and K.shape[0] == T.shape[0])
 
 
-def _recognize_sim3(model, input, params, group, robust, solver, sparse, weight):
-    """A Sim3 pose graph takes the Sim3 route when an iterative solve was asked for (solver=PCG()/CG() or sparse=True), the
-    one trainable parameter is an (N,8) Sim3 Parameter on a CUDA device, the input is (edges (E,2) in range, Sim3 Z (E,8)) of
-    the parameter's dtype and device, there are no information matrices and no process group, and the model is the
-    built-in PoseGraph or its output equals the Sim3 pose-graph residual row by row (_same_residuals)."""
+def _recognize_lie_pgo(model, input, params, group, robust, solver, sparse, weight):
+    """A pose graph on Sim3 or SO3 nodes takes its node-ordered route (Sim3PGOProblem / SO3PGOProblem, chosen by the
+    parameter's ltype) when an iterative solve was asked for (solver=PCG()/CG() or sparse=True), the one trainable
+    parameter is an (N,D) Parameter of that group on a CUDA device, the input is (edges (E,2) in range, Z (E,D) of the same
+    group) of the parameter's dtype and device, there are no information matrices and no process group, and the model is
+    the built-in PoseGraph or its output equals the pose-graph residual row by row (_same_residuals)."""
     from .solver import CG
     from ..module.pgo import PoseGraph
     P = params[0]
+    ltype = P.ltype
     if not (isinstance(solver, CG) or sparse) or weight is not None or group is not None:
         return None
     if not (isinstance(P, Parameter) and P.is_cuda and P.dim() == 2 and P.dtype in (torch.float32, torch.float64)):
@@ -848,8 +879,8 @@ def _recognize_sim3(model, input, params, group, robust, solver, sparse, weight)
         return None
     edges, Z = input
     if not (torch.is_tensor(edges) and edges.dtype in (torch.int64, torch.int32) and edges.dim() == 2 and edges.shape[1] == 2
-            and edges.device == P.device and isinstance(Z, LieTensor) and Z.ltype is Sim3_type
-            and Z.shape == (edges.shape[0], 8) and Z.dtype == P.dtype and Z.device == P.device):
+            and edges.device == P.device and isinstance(Z, LieTensor) and Z.ltype is ltype
+            and Z.shape == (edges.shape[0], ltype.D) and Z.dtype == P.dtype and Z.device == P.device):
         return None
     tol = solver.tol if isinstance(solver, CG) else 1e-8
     maxiter = solver.maxiter if isinstance(solver, CG) else None
@@ -858,9 +889,22 @@ def _recognize_sim3(model, input, params, group, robust, solver, sparse, weight)
             return None
         if not _in_range(edges, P.shape[0]):
             raise IndexError("PoseGraph: edge index out of range")
-    elif not (_in_range(edges, P.shape[0]) and _same_residuals(model, input, params, (edges.shape[0], 7), group)):
+    elif not (_in_range(edges, P.shape[0]) and _same_residuals(model, input, params, (edges.shape[0], ltype.K), group)):
         return None
-    return Sim3PGOProblem(model, edges, Z, _input_key(input), robust, tol, maxiter, param=P)
+    return _LIE_PGO[ltype](model, edges, Z, _input_key(input), robust, tol, maxiter, param=P)
+
+
+_LIE_PGO = {Sim3_type: Sim3PGOProblem, SO3_type: SO3PGOProblem}
+
+
+def recognize_so3_graph(model, input, params, group=None, robust=(0, 1.0), solver=None, sparse=False, weight=None):
+    """SO3PGOProblem for an SO3 pose graph (rotation averaging) under the conditions of _recognize_lie_pgo, else None.
+    `recognize` keeps returning None for SO3 graphs, as it always has: the LM asks for this family only where it would
+    otherwise build per-residual blocks (an iterative solve, no weight), which is where the SO3 route replaces them."""
+    params = [p for p in params if p.requires_grad]
+    if not (len(params) == 1 and getattr(params[0], 'ltype', None) is SO3_type):
+        return None
+    return _recognize_lie_pgo(model, input, params, group, robust, solver, sparse, weight)
 
 
 def _recognize_bal(model, input, params, group, robust, solver, sparse, weight):
@@ -895,7 +939,7 @@ def _recognize_bal(model, input, params, group, robust, solver, sparse, weight):
 def _family_residuals(input, params):
     """Row-wise residuals of the family the shapes point at, from the *original* (unsorted) inputs with ordinary
     LieTensor ops — an independent restatement used only to verify a user module at recognition time."""
-    T = LieTensor(params[0].detach(), ltype=params[0].ltype)      # SE3, or Sim3 for the Sim3 pose graph
+    T = LieTensor(params[0].detach(), ltype=params[0].ltype)      # SE3, or Sim3 / SO3 for those pose graphs
     if len(params) == 2:                                          # bundle adjustment
         obs, ci, pi_ = input
         y = T[ci.long()].Act(params[1].detach()[pi_.long()])
@@ -972,7 +1016,7 @@ def recognize(model, input, params, group=None, robust=(0, 1.0), solver=None, sp
     """Return a structured problem for (model, input) or None (-> generic dense route)."""
     params = [p for p in params if p.requires_grad]
     if len(params) == 1 and getattr(params[0], 'ltype', None) is Sim3_type:
-        return _recognize_sim3(model, input, params, group, robust, solver, sparse, weight)
+        return _recognize_lie_pgo(model, input, params, group, robust, solver, sparse, weight)
     if weight is not None and not _pgo_weight(weight, input):
         return None
     from ..module.ba import BundleAdjustment
