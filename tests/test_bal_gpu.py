@@ -158,7 +158,8 @@ def scipy_reduced_solve(b, ci, pi_, scale):
 
 
 @pytest.mark.parametrize("dt", [torch.float64, torch.float32])
-@pytest.mark.parametrize("C", [300, 5000])           # both sides of kVecSmallRows (4096 cameras)
+# cg_vec_small_kernel<256> (C <= 2048), cg_vec_small_kernel<512> (2048 < C <= kVecSmallRows = 4096), the grid path (C > 4096)
+@pytest.mark.parametrize("C", [300, 3000, 5000])
 def test_pcg_solution_matches_scipy(dt, C):
     d = B.problem(7, C=C, P=2 * C, M=8 * C)
     lay = Layout(d, dt)
